@@ -1,18 +1,22 @@
 #!/usr/bin/env python
-"""bench.py — the Decoder hot path on B200: log lines/s and GB/s parsed, with roofline + CPU baseline.
+"""bench.py — the Decoder hot path on H100: log lines/s and GB/s parsed, with roofline + CPU baseline.
 
     python bench.py --gpus N --steps K --warmup W [--format rfc5424|ltsv|gelf|rfc3164|mixed] [--lines L] [--impl reference]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the parse kernel over one synthetic batch that is already resident in HBM
 (BASELINE.json configs[1]: 10 M RFC5424 lines, mean 180 B, per GPU).  `e2e` is the same metric through
 the reference-facing C-ABI call fg_decode_batch() with HOST buffers (pinned H2D + kernels + D2H inside
 the timed region).  For N>1 every rank owns one GPU and an independent shard of lines (weak scaling,
 no collective on the parse path); time is the max over ranks.  `--impl reference` times the CPU
-restatement of the reference decoders (oracle/) on the host cores for the same workload.
+restatement of the reference decoders (oracle/) on the host cores for the same workload.  `--dump-outputs DIR` writes
+what the last timed step computed for a fixed, seeded sample of the lines as DIR/<name>.npy (float64), so that two builds
+can be compared output for output on identical inputs.
 """
 from __future__ import annotations
 
 import argparse
+import hashlib
 import json
 import os
 import subprocess
@@ -45,11 +49,11 @@ def hbm_peak() -> tuple[float, str]:
     try:
         return float(json.loads(p.read_text())["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -154,6 +158,49 @@ def oracle_config(pyoracle, fmt_name: str, typed: bool):
     if fmt_name == "rfc3164":
         return pyoracle.Rfc3164Config(RFC3164_YEAR)
     return None
+
+
+DUMP_SEED = 20240
+DUMP_BLOCK = 1024  # lines per sampled block
+
+
+def dump_outputs(out_dir: str, prefix: str, dec, res, data, offs, blocks: int) -> None:
+    """What a caller of the decoder receives for `blocks` seeded blocks of DUMP_BLOCK consecutive lines (every line if the
+    batch is smaller), as float64 columns: the line number, ts, meta (status | facility << 8 | severity << 16 | flags << 24),
+    (offset, length) of each header span, the SD entry count and a 48-bit digest of the line's materialised Record (the
+    canonical dump, which covers SD names and values).  Offsets into the batch arena depend on the order the CTAs ran in, so
+    they are written as -1; the digest still covers the text they point to."""
+    import numpy as np
+    import flowgger_b200 as fb
+    n = res.n
+    nblk = n // DUMP_BLOCK
+    if nblk <= blocks:
+        ranges = [(0, n)]
+    else:
+        starts = np.sort(np.random.default_rng(DUMP_SEED).choice(nblk, blocks, replace=False)) * DUMP_BLOCK
+        ranges = [(int(s), int(s) + DUMP_BLOCK) for s in starts]
+    idx = np.concatenate([np.arange(lo, hi) for lo, hi in ranges])
+    if dec.fmt == fb.FMT_RFC5424:
+        spans = res.spans5424(offs)
+    else:
+        spans = {k: getattr(res, k) for k in ("hostname", "appname", "procid", "msgid", "msg", "full_msg", "sd")}
+    meta = res.meta[idx]
+    cols = {"line": idx, "ts": res.ts[idx], "meta": meta, "sd_count": spans["sd"][idx, 1]}
+    for k in ("hostname", "appname", "procid", "msgid", "msg", "full_msg"):
+        if len(spans[k]) == 0:
+            continue  # a column this format does not produce
+        s = spans[k][idx].astype(np.float64)
+        if k == "msg" and dec.fmt == fb.FMT_RFC3164:
+            s[((meta >> 24) & 0x40) != 0, 0] = -1  # FG_FLAG_MSG_ARENA
+        cols[k] = s
+    digest = []
+    for lo, hi in ranges:
+        buf, o = dec.dump(res, data, offs, nthreads=min(os.cpu_count() or 8, 32), lo=lo, hi=hi)
+        digest += [int.from_bytes(hashlib.blake2b(buf[o[i]:o[i + 1]], digest_size=6).digest(), "little") for i in range(hi - lo)]
+    cols["record_digest"] = np.asarray(digest, dtype=np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in cols.items():
+        np.save(os.path.join(out_dir, f"{prefix}{k}.npy"), np.ascontiguousarray(v, dtype=np.float64))
 
 
 def run_reference(args) -> None:
@@ -269,6 +316,9 @@ def run_mixed(args) -> None:
     wall = reduce(time.perf_counter() - t0, torch.distributed.ReduceOp.MAX if dist else None)
     clocks = sampler.stop() if rank == 0 else None
     launches = sum(d[1].kernel_launches() for d in decs) - launches0
+    if args.dump_outputs and rank == 0:
+        for k, (fmt_name, dec, hb, ho, n, nb) in enumerate(decs):
+            dump_outputs(args.dump_outputs, f"{k}_{fmt_name}_", dec, dec.download(), hb, ho, blocks=256 // len(decs))
     per_gpu = tot_lines / (wall / args.steps)
     total_lines = reduce(float(tot_lines), torch.distributed.ReduceOp.SUM if dist else None)
     total_bytes = reduce(float(tot_bytes), torch.distributed.ReduceOp.SUM if dist else None)
@@ -311,7 +361,7 @@ def run_mixed(args) -> None:
             "config": {"workload": f"Mixed RFC5424+GELF stream, runs of {RUN} lines, {tot_lines} lines per GPU ({n5} RFC5424 + {ng} GELF), "
                                    f"{world} GPU(s) (BASELINE.json configs[4] = 100 M lines over 8 GPUs)",
                        "lines_per_gpu": tot_lines, "bytes_per_gpu": tot_bytes, "sub_batches": [(f, n) for f, _, _, _, n, _ in decs],
-                       "parallelism": f"line shards x{world}, no collective", "l2": "every sub-batch >> 126 MB L2"},
+                       "parallelism": f"line shards x{world}, no collective", "l2": "every sub-batch >> 50 MB L2"},
             "kernel_ms": {k: v / args.steps for k, v in kms.items()},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "of": peak_kind,
                          "traffic": None, "kernel": "parse_gelf_kernel + post_gelf_kernel (dominant: %.1f of %.1f ms/step)" % (g_ms, (kms["gelf"] + kms["rfc5424"]) / args.steps)},
@@ -352,7 +402,13 @@ def main() -> None:
     ap.add_argument("--split", action="store_true", help="also time fg_split_decode (device-side framing + UTF-8 validation, N1)")
     ap.add_argument("--ltsv-typed", action="store_true", help="LTSV with the 4-entry typed schema + suffixes (C4, second run)")
     ap.add_argument("--encode", action="store_true", help="also time fg_decode_encode_gelf (decode + GELF encode fused on the device, N2)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (a seeded sample of the lines) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of the CUDA decoder; the reference arm returns none")
     if args.format == "mixed":
         if args.lines <= 0:
             args.lines = 12_500_000
@@ -448,12 +504,14 @@ def main() -> None:
 
     # the dominant kernel alone (RFC5424: parse5424_kernel, without post5424_kernel), CUDA events around it, single steps
     dom = []
-    for _ in range(max(args.steps, 10)):
+    for _ in range(args.steps):
         dec.parse_resident()
         dom.append(dec.last_dominant_kernel_ms())
     dom_ms = max_over_ranks(sum(dom) / len(dom))
     res = dec.download()
     n_err = int((res.status != 0).sum())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, "", dec, res, h_bytes, h_offs, blocks=256)
     n_entries = res.n_entries
     if fmt == 0:
         # compact results: 32-byte row per line + 8-byte side-table rows + the arena of unescaped values (+ rare wide rows)
@@ -550,17 +608,6 @@ def main() -> None:
     if rank == 0:
         peak, peak_kind = hbm_peak()
         achieved = (b_read / 1e9) / (dom_ms / 1e3)
-        # dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel per launch, from the committed ncu capture of
-        # THIS kernel build (profiles/traffic.json names the build it was taken from); scaled to this run's line count
-        traffic = None
-        tp = REPO / "profiles" / "traffic.json"
-        if tp.exists():
-            try:
-                t = json.loads(tp.read_text()).get(fmt_name)
-                if t and t.get("build") == fb.build_info():
-                    traffic = int(t["dram_bytes_per_line"] * n)
-            except Exception:
-                traffic = None
         line = {
             "metric": "log lines/sec parsed (%s)" % fmt_name.upper(), "value": value, "unit": "lines/s",
             "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_per_step,
@@ -569,10 +616,10 @@ def main() -> None:
             "config": {"workload": workload_name(fmt_name, n), "lines_per_gpu": n, "bytes_per_gpu": nbytes,
                        "mean_line_bytes": round(nbytes / n, 2), "error_rows": n_err, "sd_entries": n_entries,
                        "parallelism": f"line shards x{world}, no collective", "host_affinity_rank0": numa,
-                       "l2": "input per step (%.2f GB) >> 126 MB L2, no flush needed" % (nbytes / 1e9)},
+                       "l2": "input per step (%.2f GB) >> 50 MB L2, no flush needed" % (nbytes / 1e9)},
             "kernel_ms": k_avg_ms,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "of": peak_kind, "traffic": traffic,
+                         "of": peak_kind, "traffic": None,
                          "kernel": {0: "parse5424_kernel", 1: "parse_ltsv_kernel", 2: "parse_gelf_kernel + post_gelf_kernel", 3: "parse3164_kernel"}[fmt],
                          "kernel_ms": dom_ms, "step_ms": k_avg_ms, "step_frac": (b_read / 1e9) / (k_avg_ms / 1e3) / peak,
                          "note": "achieved = algorithmic bytes / CUDA-event time of the dominant kernel alone (single steps); "

@@ -1,6 +1,6 @@
-"""flowgger_b200 — B200-native batched log-line decoder (RFC5424 / LTSV / GELF bytes -> Record).
+"""flowgger_b200 — H100-native batched log-line decoder (RFC5424 / LTSV / GELF bytes -> Record).
 
-Drop-in for flowgger's Decoder stage (`/root/reference/src/flowgger/decoder/mod.rs:44-46`): the
+Drop-in for flowgger's Decoder stage (`flowgger src/flowgger/decoder/mod.rs:44-46`): the
 product is the C-ABI shared library `lib/libflowgger_cuda.so` (see `include/flowgger_cuda.h`); this
 Python package is a thin ctypes binding over it used by the tests and `bench.py`.  There is no CPU
 fallback: importing works anywhere, but constructing a decoder needs the built library and a GPU.

@@ -1,4 +1,4 @@
-"""Build the in-tree native libraries (sm_100a only).
+"""Build the in-tree native libraries (sm_90a only: H100).
 
     python -m flowgger_b200.build [--force]
 
@@ -22,7 +22,7 @@ LIB = ROOT / "lib"
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-O3",
     "--fmad=false",          # keep IEEE double semantics explicit (timestamp recipe)
@@ -37,6 +37,17 @@ def _newer(target: Path, sources: list[Path]) -> bool:
         return True
     t = target.stat().st_mtime
     return any(s.stat().st_mtime > t for s in sources)
+
+
+def _build(target: Path, sources: list[Path], cmd: list[str], force: bool) -> None:
+    """Run `cmd` when `target` is missing, older than a source, or was built by another command line (a change of
+    NVCC_FLAGS, e.g. the architecture, rebuilds even when no source changed).  The command line is kept next to the
+    target in `<target>.cmd`."""
+    stamp = target.with_name(target.name + ".cmd")
+    line = " ".join(cmd).replace(str(REPO), ".")  # a moved or copied tree keeps its build
+    if force or _newer(target, sources) or not stamp.exists() or stamp.read_text() != line:
+        _run(cmd)
+        stamp.write_text(line)
 
 
 def _run(cmd: list[str]) -> None:
@@ -57,9 +68,8 @@ def build_cuda(force: bool = False) -> Path:
     target = LIB / "libflowgger_cuda.so"
     srcs = sorted(CSRC.glob("*.cu")) + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + [
         REPO / "include" / "flowgger_cuda.h"]
-    if force or _newer(target, srcs):
-        cus = [str(p) for p in sorted(CSRC.glob("*.cu"))]
-        _run([NVCC, *NVCC_FLAGS, "-shared", "-o", str(target), *cus, "-I", str(REPO / "include")])
+    cus = [str(p) for p in sorted(CSRC.glob("*.cu"))]
+    _build(target, srcs, [NVCC, *NVCC_FLAGS, "-shared", "-o", str(target), *cus, "-I", str(REPO / "include")], force)
     return target
 
 
@@ -69,9 +79,8 @@ def build_host(force: bool = False) -> Path | None:
         return None
     target = LIB / "libflowgger_host.so"
     srcs = sorted(hdir.glob("*.cpp")) + sorted(hdir.glob("*.hpp")) + [REPO / "include" / "flowgger_cuda.h"]
-    if force or _newer(target, srcs):
-        _run([CXX, *CXX_FLAGS, "-shared", "-o", str(target), *[str(p) for p in sorted(hdir.glob("*.cpp"))],
-              "-I", str(REPO / "include"), f"-L{LIB}", "-lflowgger_cuda", "-Wl,-rpath,$ORIGIN"])
+    _build(target, srcs, [CXX, *CXX_FLAGS, "-shared", "-o", str(target), *[str(p) for p in sorted(hdir.glob("*.cpp"))],
+                          "-I", str(REPO / "include"), f"-L{LIB}", "-lflowgger_cuda", "-Wl,-rpath,$ORIGIN"], force)
     return target
 
 
@@ -81,8 +90,7 @@ def build_gen(force: bool = False) -> Path | None:
         return None
     target = LIB / "libfg_gen.so"
     srcs = sorted(gdir.glob("*.cpp")) + sorted(gdir.glob("*.hpp"))
-    if force or _newer(target, srcs):
-        _run([CXX, *CXX_FLAGS, "-shared", "-o", str(target), *[str(p) for p in sorted(gdir.glob("*.cpp"))]])
+    _build(target, srcs, [CXX, *CXX_FLAGS, "-shared", "-o", str(target), *[str(p) for p in sorted(gdir.glob("*.cpp"))]], force)
     return target
 
 

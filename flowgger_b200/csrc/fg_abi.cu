@@ -27,7 +27,7 @@
 
 namespace {
 
-// The reference's `&'static str` for every status (file:line in /root/reference/src/flowgger/decoder/)
+// The reference's `&'static str` for every status (file:line in flowgger src/flowgger/decoder/)
 const char* kErrorStrings[FG_ST_COUNT] = {};
 struct ErrorTableInit {
     ErrorTableInit() {
@@ -193,6 +193,7 @@ struct fg_ctx {
     int64_t launches = 0;
     int max_tile = 0;   // LTSV / GELF staging tile limit
     int max_tile5 = 0;  // RFC5424: tile + bitmap must fit the opt-in shared memory
+    int num_sms = 0;    // of the device: the post kernels' fixed grids stride over their work lists with a few CTAs per SM
 };
 
 namespace {
@@ -382,7 +383,7 @@ int ensure_format(fg_ctx* c, int fmt) {
 int pick_tile(const fg_ctx* c, size_t total_bytes, int n, int fmt) {
     const double mean = n > 0 ? (double)total_bytes / n : 0.0;
     const long lines = fg::lines_per_cta(fmt), gran = 8 * lines;  // 1 KiB steps for 128-line CTAs, 512 B for 64
-#ifndef FG_TILE_SLACK_PCT  // head room of the tile over the mean span of a CTA's lines (profiles/variants.sh tries others)
+#ifndef FG_TILE_SLACK_PCT  // head room of the tile over the mean span of a CTA's lines (-DFG_TILE_SLACK_PCT=... tries others)
 #define FG_TILE_SLACK_PCT 102
 #endif
     long t = (long)(mean * lines * (FG_TILE_SLACK_PCT / 100.0)) + gran;
@@ -444,6 +445,7 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
         P.bad_offsets = c->d_k + kBadFlag;
         P.line_invalid = invalid;
         P.strip_eol = strip_eol;
+        P.num_sms = c->num_sms;
         FG_CUDA(c, cudaMemsetAsync(c->d_k + fg::K5_ESC_LIST, 0, 8, s));  // the two work lists are per launch
         FG_CUDA(c, fg::launch_parse5424(P, s, time_dominant ? c->ev_dom0 : nullptr, time_dominant ? c->ev_dom1 : nullptr));
         c->launches += 2;  // parse5424_kernel + post5424_kernel
@@ -455,6 +457,7 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
     P.n = n;
     P.line0 = line0;
     P.tile_bytes = tile;
+    P.num_sms = c->num_sms;
     uint8_t* r = c->d_rows;
     P.ts = (double*)(r + col_off(c, C_TS)) + line0;
     P.meta = (uint32_t*)(r + col_off(c, C_META)) + line0;
@@ -779,7 +782,7 @@ int fg_create(const fg_config* cfg, fg_ctx** out) {
     if (c->max_bytes > 0x7FFFFFC0ull) c->max_bytes = 0x7FFFFFC0ull;  // int32 offsets
     c->max_lines = cfg->max_batch_lines > 0 ? cfg->max_batch_lines : (2 << 20);
     c->max_lines = (c->max_lines + 63) & ~63;  // keeps every row column 256-byte aligned
-    c->chunk_lines = cfg->chunk_lines > 0 ? cfg->chunk_lines : (512 << 10);  // measured: 246 / 258 / 258 M lines/s e2e at 128 Ki / 512 Ki / 1 Mi lines per chunk (profiles/r2_notes.md)
+    c->chunk_lines = cfg->chunk_lines > 0 ? cfg->chunk_lines : (512 << 10);
     c->chunk_lines = (c->chunk_lines + 127) / 128 * 128;  // a multiple of every kernel's lines per CTA
     c->r3164_year = cfg->rfc3164_year;
     if (cfg->tzdir) c->tzdir = cfg->tzdir;
@@ -797,6 +800,7 @@ int fg_create(const fg_config* cfg, fg_ctx** out) {
     FG_CREATE_CUDA(cudaGetDeviceProperties(&prop, c->device));
     c->max_tile = (int)std::min<size_t>(prop.sharedMemPerBlockOptin - 1024, 200 * 1024);
     c->max_tile &= ~1023;
+    c->num_sms = prop.multiProcessorCount;
     c->max_tile5 = (int)(((size_t)c->max_tile - 1024) * 8 / 9) & ~1023;  // tile + tile/8 bitmap + static shared memory
     FG_CREATE_CUDA(fg::configure_kernels(c->max_tile, c->max_tile5));
     FG_CREATE_CUDA(cudaStreamCreateWithFlags(&c->s_h2d, cudaStreamNonBlocking));

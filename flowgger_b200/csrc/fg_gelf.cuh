@@ -1,7 +1,7 @@
 // fg_gelf.cuh — one GELF (JSON) line -> Record fields, on device.
 //
-// B200-native replacement for GelfDecoder::decode
-// (/root/reference/src/flowgger/decoder/gelf_decoder.rs:34-125).  The JSON semantics are those of the
+// H100-native replacement for GelfDecoder::decode
+// (flowgger src/flowgger/decoder/gelf_decoder.rs:34-125).  The JSON semantics are those of the
 // un-vendored serde_json ~0.8 the reference links (Cargo.toml:51), restated from its published source:
 //   de.rs   parse_value / parse_integer / parse_long_integer / parse_number / parse_decimal /
 //           parse_exponent / parse_exponent_overflow / visit_f64_from_parts, MapVisitor / SeqVisitor

@@ -1,6 +1,6 @@
 // fg_gelf_encode.cu — the stage AFTER the decoder, fused on the device: Record -> GELF JSON bytes (SURVEY.md §8(f) N2).
 //
-// B200-native replacement for GelfEncoder::encode (/root/reference/src/flowgger/encoder/gelf_encoder.rs:59-115), which
+// H100-native replacement for GelfEncoder::encode (flowgger src/flowgger/encoder/gelf_encoder.rs:59-115), which
 // every splitter calls right after Decoder::decode (splitter/line_splitter.rs:50-52).  The JSON text is what
 // serde_json "~0.8" `to_vec` prints for the BTreeMap the reference builds: keys in byte order, a later insert replaces
 // an earlier one (SD pairs replace fixed fields, output.gelf_extra replaces everything), compact separators, strings
@@ -198,8 +198,8 @@ __device__ __forceinline__ bool load_pair(const GelfEncodeParams& P, const ByteS
 enum { GF_APP = 0, GF_FULL, GF_HOST, GF_LEVEL, GF_PROC, GF_SDID, GF_SHORT, GF_TS, GF_VERSION, GF_EXTRA = 100 };
 
 // ---- a record = a short list of segments, then ONE byte loop -------------------------------------------------------
-// Emitting field by field with a byte loop per field made every lane of a warp sit in a different loop (4 of 32 lanes
-// active, 1100 warp-instructions per record, profiles/r2c_ncu_gelf_write.txt).  Now a lane first lists its record as
+// Emitting field by field with a byte loop per field made every lane of a warp sit in a different loop, a few of 32
+// lanes active at a time.  Now a lane first lists its record as
 // segments (pointer, length, copy / JSON-escape) — short, divergent — and then all 32 lanes run the SAME loop that
 // produces one output byte per iteration from the current segment.
 struct Seg {
@@ -317,7 +317,7 @@ struct PairCursor {
 // `num` (>= 32 bytes, owned by the caller) receives the text of Record.ts and is referenced by a segment.
 // Called by ALL 32 lanes (`live` = this lane has a record).  The loop runs over the STATIC items, which are the same for
 // every record, so the lanes of a warp stay on the same item (the first version merged pair by pair per lane: the lanes
-// drifted apart by their pair counts and every static item ran ~3 lanes wide, profiles/r2_notes.md); the SD pairs that
+// drifted apart by their pair counts and every static item ran a few lanes wide); the SD pairs that
 // sort before the current item are emitted by an inner loop whose trip count is the warp's maximum.
 __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, bool live, uint8_t* num,
                                                SegList& L) {
@@ -407,8 +407,7 @@ __device__ __forceinline__ uint32_t json_escape_flags4(uint32_t w) {
 }
 
 // The warp-uniform loop: per lane and iteration FOUR output bytes when the segment has them and none needs an escape, else
-// one.  `live` = this lane has a record to emit.  (One byte per iteration cost ~65 instructions per byte: 1570
-// warp-instructions per record, profiles/r2_notes.md.)
+// one.  `live` = this lane has a record to emit.  (One byte per iteration spends the loop's bookkeeping on every byte.)
 template <class Sink>
 __device__ __forceinline__ void run_segments(const SegList& L, bool live, Sink& s) {
     int si = 0, k = 0, len = 0;

@@ -1,7 +1,7 @@
 // fg_gelffast.cuh — GELF on the bitmap pipeline, MEMBER-parallel, for REGULAR lines; everything else goes to the exact
 // parser of fg_gelf.cuh.
 //
-// B200-native replacement for GelfDecoder::decode (/root/reference/src/flowgger/decoder/gelf_decoder.rs:34-125).  A regular
+// H100-native replacement for GelfDecoder::decode (flowgger src/flowgger/decoder/gelf_decoder.rs:34-125).  A regular
 // line is what every GELF sender emits: ONE flat JSON object
 //     { "key" : value , "key" : value ... }        value = string | number | true | false | null
 // with nothing but spaces between the tokens, no escape inside a key, no raw control byte anywhere, at most
@@ -20,8 +20,7 @@
 //            string escapes, literals; numbers are listed and go through json_number in a dense second pass.
 //   phase 2  gf_finish: one thread per line sorts the members by key (8-byte prefix first), keeps the last duplicate and
 //            applies the per-key rules of gelf_decoder.rs:51-107.
-// (Walking a line member by member in lock step — the first two versions — cost 1258 / 1392 warp-instructions per line
-//  and was slower than the round-1 tokenizer; profiles/r2_notes.md.)
+// (Walking a line member by member in lock step — the first two versions — was slower than the round-1 tokenizer.)
 #pragma once
 #include "fg_common.cuh"
 #include "fg_gelf.cuh"
@@ -112,7 +111,7 @@ FG_DEV uint32_t gf_clip(uint32_t w, int word, int lo, int hi) {
 // word.
 FG_DEV int gf_line_commas(const uint32_t* bmQ, const uint32_t* bmB, const uint32_t* bmP, int ls, int le, uint16_t* cuts, int cap, bool act) {
     // All lanes of the warp call (act = this lane has a line): the word loop and the comma loop run in lock step — written
-    // with plain loops and early returns the lanes of a warp drifted apart and ran one at a time (profiles/r2_notes.md).
+    // with plain loops and early returns the lanes of a warp drifted apart and ran one at a time.
     const bool run = act && le > ls;
     const int w0 = ls >> 5, w1 = run ? (le - 1) >> 5 : w0 - 1;
     uint32_t prev_escaped = 0u;    // bit 0: the first byte of this word is escaped by a run ending in the previous word

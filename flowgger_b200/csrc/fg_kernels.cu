@@ -1,4 +1,4 @@
-// fg_kernels.cu — configuration and dispatch of the batched parse kernels (sm_100a).
+// fg_kernels.cu — configuration and dispatch of the batched parse kernels (sm_90a).
 //
 // RFC5424, LTSV and GELF run on the same pipeline (DESIGN.md §3), each in its own file; RFC3164 shares the staging only:
 //   RFC5424  fg_parse5424.cu   parse5424_kernel + post5424_kernel
@@ -55,7 +55,7 @@ cudaError_t launch_parse(int fmt, const ParseParams& p, cudaStream_t stream) {
 }
 
 const char* kernel_build_info() {
-    return "flowgger_b200 parse kernels: sm_100a, structural bitmaps + bit-walk over TMA-bulk-staged CTA tiles, "
+    return "flowgger_b200 parse kernels: sm_90a, structural bitmaps + bit-walk over TMA-bulk-staged CTA tiles, "
            "kernels=[parse5424_kernel, post5424_kernel, gelf_size_kernel, gelf_write_kernel, parse_ltsv_kernel, parse_gelf_kernel, post_gelf_kernel, parse3164_kernel]";
 }
 

@@ -78,6 +78,7 @@ struct ParseParams {
     // GELF: launch-relative numbers of the lines the fast walker hands to the exact parser (post_gelf_kernel)
     uint32_t* slow_list;
     uint32_t* slow_count;
+    int32_t num_sms;          // SMs of the context's device: sizes the fixed grid of post_gelf_kernel
     LtsvDeviceConfig ltsv;
     R3164DeviceConfig r3164;
 };
@@ -127,6 +128,7 @@ struct Parse5424Params {
     const uint32_t* bad_offsets;  // see ParseParams
     const uint8_t* line_invalid;  // split mode, or nullptr
     int32_t strip_eol;
+    int32_t num_sms;         // SMs of the context's device: sizes the fixed grid of post5424_kernel
 };
 
 // parse5424_kernel + post5424_kernel; when given, the two events bracket the parse kernel alone (roofline measurement)
@@ -168,10 +170,10 @@ cudaError_t launch_gelf_encode(const GelfEncodeParams& p, void* d_scan_temp, siz
 size_t gelf_scan_temp_bytes(int n);
 
 // RFC5424 (short lines, staged tile): 64-line CTAs — tile waits and barriers half as wide as with 128 lines
-#ifndef FG_R5_LINES  // profiles/variants.sh builds other shapes with -DFG_R5_LINES / -DFG_R5_MINB for A/B runs
+#ifndef FG_R5_LINES  // other shapes build with -DFG_R5_LINES / -DFG_R5_MINB for A/B runs
 #define FG_R5_LINES 64
 #endif
-#ifndef FG_R5_MINB  // 16 CTAs/SM (64 registers, tile slack 2 %) measured 2 % faster than 14 (71 registers, 10 %): profiles/r2_notes.md
+#ifndef FG_R5_MINB  // 16 CTAs/SM: 64 registers, tile slack 2 %
 #define FG_R5_MINB 16
 #endif
 constexpr int kRfc5424LinesPerCta = FG_R5_LINES;
@@ -200,7 +202,7 @@ constexpr int kGelfCtasPerSm = 3;  // tile (~34 KB at 520 B/line) + bitmap + slo
 constexpr int kGelfStageSlots = kGelfLinesPerCta * 16;
 constexpr int kGelfMaxTile = 65024;
 // RFC3164 (fg_parse3164.cu): 64 lines and 64 threads per CTA, one thread per line over the staged tile
-#ifndef FG_R3_LINES  // profiles/r2_rfc3164_variants.sh builds other shapes for A/B runs
+#ifndef FG_R3_LINES  // other shapes build with -DFG_R3_LINES / -DFG_R3_MINB for A/B runs
 #define FG_R3_LINES 64
 #endif
 #ifndef FG_R3_MINB

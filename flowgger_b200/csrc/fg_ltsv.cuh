@@ -1,7 +1,7 @@
 // fg_ltsv.cuh — one LTSV line -> Record fields, on device.
 //
-// B200-native replacement for LTSVDecoder::decode
-// (/root/reference/src/flowgger/decoder/ltsv_decoder.rs:87-221) and its helpers
+// H100-native replacement for LTSVDecoder::decode
+// (flowgger src/flowgger/decoder/ltsv_decoder.rs:87-221) and its helpers
 // rfc3339_to_unix :224-229, english_time_to_unix[_with_subsecond] :231-254,
 // unix_strtime_to_unix :256-261, parse_ts :263-267.  Schema / suffix configuration
 // (LTSVDecoder::new :24-83) arrives as flat device arrays (LtsvDeviceConfig).

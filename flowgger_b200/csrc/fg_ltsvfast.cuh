@@ -1,7 +1,7 @@
 // fg_ltsvfast.cuh — LTSV on the bitmap pipeline, PART-parallel: the tab-separated parts of a line are independent of each
 // other, so the unit of work of the hot phase is a part, not a line.
 //
-// B200-native replacement for LTSVDecoder::decode (/root/reference/src/flowgger/decoder/ltsv_decoder.rs:87-221); the
+// H100-native replacement for LTSVDecoder::decode (flowgger src/flowgger/decoder/ltsv_decoder.rs:87-221); the
 // value parsers (parse_ts :263-267, the typed schema values :138-195) are the ones of fg_ltsv.cuh, called on tile bytes.
 //
 //   stage 1  lt_tab16: every thread takes 32-byte granules of the flat tile (two LDS.128, all 32 lanes busy) and writes one
@@ -11,8 +11,7 @@
 //   parts    lt_part: one thread per SLOT, for all slots of the CTA round, 256 threads wide: the key ends at the first ':'
 //            (splitn(2, ':') :95, a SWAR test on the first 8 key bytes), the four reserved keys are recognised from
 //            those 8 bytes, everything else becomes a packed side-table row in the slot.  No loop over a line, no lock step,
-//            no lane waits for a longer line (round 2 measured the thread-per-line walk at 315 warp-instructions per line
-//            with 8 warps per SM; profiles/r2_notes.md).
+//            no lane waits for a longer line (a thread-per-line walk makes every lane wait for the warp's longest line).
 //   lines    lt_finish_line: one thread per line parses the (last) `time` and `level` values, picks the first failing part
 //            and builds the row.
 // Lines that need the reference's sequential semantics beyond that — a repeated `time` or `level` key — and lines that do

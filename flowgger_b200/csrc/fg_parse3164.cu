@@ -1,4 +1,4 @@
-// fg_parse3164.cu — the RFC3164 decoder on sm_100a (SURVEY.md §8(f) N3): bytes -> row columns (+ re-joined messages).
+// fg_parse3164.cu — the RFC3164 decoder on sm_90a (SURVEY.md §8(f) N3): bytes -> row columns (+ re-joined messages).
 //
 //   parse3164_kernel   one CTA = 64 consecutive lines, 64 threads.
 //     (1) thread 0 issues ONE TMA bulk copy (cp.async.bulk, SASS UBLKCP) of the lines' contiguous byte span into the

@@ -1,4 +1,4 @@
-// fg_parse5424.cu — the RFC5424 hot path on sm_100a: bytes -> compact 32-byte rows + 8-byte side-table entries.
+// fg_parse5424.cu — the RFC5424 hot path on sm_90a: bytes -> compact 32-byte rows + 8-byte side-table entries.
 //
 //   parse5424_kernel     one CTA = LINES consecutive lines.  (1) thread 0 issues ONE TMA bulk copy (cp.async.bulk, SASS
 //                        UBLKCP) of the CTA's contiguous byte span into the shared-memory tile; (2) all threads sweep the tile
@@ -83,8 +83,7 @@ __global__ void __launch_bounds__(LINES, MINB) parse5424_kernel(const __grid_con
 
         // ---- stage 2: one thread per line ------------------------------------------------------------------------
         // (Counting-sorting the CTA's lines by a work estimate so that a warp's 32 lines have similar pair counts was
-        //  measured: 1.56 vs 1.43 ms per step — the estimate, the two extra barriers and the scattered row stores cost
-        //  more than the shorter walks gain; profiles/r2_notes.md.)
+        //  slower: the estimate, the two extra barriers and the scattered row stores cost more than the shorter walks gain.)
         const bool active = tid < r;
         int ls = active ? o0 - base : 0;
         int le = active ? o1 - base : 0;
@@ -368,8 +367,9 @@ cudaError_t launch_parse5424(const Parse5424Params& p, cudaStream_t stream, cuda
     parse5424_kernel<kFastLines, kFastCtasPerSm><<<grid, kFastLines, parse5424_smem_bytes(p.tile_bytes), stream>>>(p);
     if (dom1) cudaEventRecord(dom1, stream);
     // the work lists live on the device (no host round trip): a fixed grid strides over them
-    const int esc_ctas = (int)min((long long)(p.n + 127) / 128, 148LL * 12);
-    const int wide_ctas = (int)min((long long)(p.n + 127) / 128, 148LL * 4);
+    const long long sms = p.num_sms;
+    const int esc_ctas = (int)min((long long)(p.n + 127) / 128, sms * 12);
+    const int wide_ctas = (int)min((long long)(p.n + 127) / 128, sms * 4);
     post5424_kernel<<<esc_ctas + wide_ctas, 128, 0, stream>>>(p, esc_ctas);
     return cudaGetLastError();
 }

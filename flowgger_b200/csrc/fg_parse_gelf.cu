@@ -1,4 +1,4 @@
-// fg_parse_gelf.cu — the GELF decoder on sm_100a: bytes -> row columns + side table, on the bitmap pipeline, member-parallel.
+// fg_parse_gelf.cu — the GELF decoder on sm_90a: bytes -> row columns + side table, on the bitmap pipeline, member-parallel.
 //
 //   parse_gelf_kernel   one CTA = 64 consecutive lines, 256 threads.  Per round:
 //     (1) ONE TMA bulk copy (cp.async.bulk, SASS UBLKCP) of the lines' contiguous byte span into the shared-memory tile;
@@ -370,7 +370,7 @@ cudaError_t launch_parse_gelf(const ParseParams& p, cudaStream_t stream) {
     const int grid = (p.n + kLines - 1) / kLines;
     parse_gelf_kernel<<<grid, kThreads, parse_gelf_smem_bytes(p.tile_bytes), stream>>>(p);
     // the work list lives on the device (no host round trip): a fixed grid strides over it
-    const int post = (int)min((long long)(p.n + 127) / 128, 148LL * 8);
+    const int post = (int)min((long long)(p.n + 127) / 128, (long long)p.num_sms * 8);
     post_gelf_kernel<<<post, 128, 0, stream>>>(p);
     return cudaGetLastError();
 }

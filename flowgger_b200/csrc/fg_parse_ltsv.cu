@@ -1,4 +1,4 @@
-// fg_parse_ltsv.cu — the LTSV decoder on sm_100a: bytes -> row columns + side table, on the bitmap pipeline, part-parallel.
+// fg_parse_ltsv.cu — the LTSV decoder on sm_90a: bytes -> row columns + side table, on the bitmap pipeline, part-parallel.
 //
 //   parse_ltsv_kernel   one CTA = 64 consecutive lines, 256 threads.  Per round:
 //     (1) thread 0 issues ONE TMA bulk copy (cp.async.bulk, SASS UBLKCP) of the lines' contiguous byte span into the

@@ -1,7 +1,7 @@
 // fg_r5fast.cuh — RFC5424 fast path: structural bitmaps + one-pair-per-step walk over a shared-memory tile.
 //
-// B200-native replacement for RFC5424Decoder::decode
-// (/root/reference/src/flowgger/decoder/rfc5424_decoder.rs:18-49) and its helpers BOM::parse :63-71,
+// H100-native replacement for RFC5424Decoder::decode
+// (flowgger src/flowgger/decoder/rfc5424_decoder.rs:18-49) and its helpers BOM::parse :63-71,
 // parse_pri_version :74-92, rfc3339_to_unix :94-99, parse_data :127-161, parse_msg :163-172,
 // parse_sd_data :174-242 — for REGULAR lines, i.e. lines of the shape every syslog sender emits:
 //     <PRI>1 TS HOST APP PROCID MSGID (-|[id name="value" name="value"][id ...]) MSG

@@ -363,10 +363,9 @@ FG_DEV void r3164_parse_line(bytes_t p, int len, const R3164DeviceConfig& cfg, R
 // ====================================================================================================================
 // The same decoder written for a WARP: r3164_parse_lockstep.
 //
-// profiles/r2r_ncu_parse3164_v1.txt: with r3164_parse_line above, the 32 lanes of a warp leave each data-dependent loop
-// (PRI digits, token lengths, ...) at different iterations and, the function being a thicket of early returns, are not
-// brought back together before its end — 3.2 of 32 lanes per issued instruction, 826 warp instructions per line, and the
-// instruction fetch cannot keep up with 32 lanes in 32 places (stall_no_instruction 8.6 per issue).  Here every lane of the
+// With r3164_parse_line above, the 32 lanes of a warp leave each data-dependent loop (PRI digits, token lengths, ...) at
+// different iterations and, the function being a thicket of early returns, are not brought back together before its end:
+// a few lanes per issued instruction, and the instruction fetch cannot keep up with 32 lanes in 32 places.  Here every lane of the
 // warp walks through the SAME sequence of phases; a lane that has nothing to do in a phase idles in it.  Every loop runs
 // until no lane of the warp needs another iteration (fg_any), and no lane returns early, so the warp is converged at
 // every phase boundary by construction.  The per-lane results are those of r3164_parse_line, statement for statement:

@@ -6,8 +6,8 @@
 // hold u16 positions), lines longer than the staging tile, and lines whose side-table rows do not fit behind the
 // cursor.  The block-scan primitives at the top are shared with the LTSV / GELF parsers.
 //
-// B200-native replacement for RFC5424Decoder::decode
-// (/root/reference/src/flowgger/decoder/rfc5424_decoder.rs:18-49) and its helpers
+// H100-native replacement for RFC5424Decoder::decode
+// (flowgger src/flowgger/decoder/rfc5424_decoder.rs:18-49) and its helpers
 // BOM::parse :63-71, parse_pri_version :74-92, rfc3339_to_unix :94-99,
 // parse_data :127-161, parse_msg :163-172, parse_sd_data :174-242.
 // The table rows carry the raw value span plus FG_EM_UNESCAPE; post5424_kernel (wide_lines) then rewrites
@@ -16,8 +16,8 @@
 // One thread owns one line.  SIMT discipline: the 32 lines of a
 // warp advance in LOCK STEP through the same phases; every data-dependent loop
 // is a warp-uniform `while (__any_sync(..))` whose body is predicated per lane,
-// so lanes never skew into different code (the first version of this kernel
-// averaged 1.95 active lanes per instruction, see profiles/r1_notes.md).
+// so lanes never skew into different code (without it the lanes of a warp
+// ran one or two at a time).
 // All 32 lanes of a warp MUST call rfc5424_parse_line (idle lanes with len = 0).
 #pragma once
 #include "fg_common.cuh"

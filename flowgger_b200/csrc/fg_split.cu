@@ -2,7 +2,7 @@
 //
 // The same kernels frame NUL-delimited streams (NulSplitter, splitter/nul_splitter.rs:18-40: `BufRead::split(0)`, the
 // delimiter is dropped, nothing else) — the delimiter byte is a launch parameter.
-// Replaces the per-record work of LineSplitter::run (/root/reference/src/flowgger/splitter/line_splitter.rs:17-25):
+// Replaces the per-record work of LineSplitter::run (flowgger src/flowgger/splitter/line_splitter.rs:17-25):
 // `BufRead::lines` (split at '\n', drop it and one preceding '\r', a last line without '\n' is still yielded) and the
 // UTF-8 check of `String` (invalid line => "Invalid UTF-8 input", line skipped).  Input: a raw byte stream resident in
 // HBM.  Output: int32 line-start offsets (line i = stream[offsets[i], offsets[i+1]) INCLUDING its terminator, which the

@@ -62,11 +62,11 @@ def cuda_lib_path() -> Path:
 def _load(name: str) -> C.CDLL:
     p = LIB_DIR / name
     if name == "libflowgger_cuda.so" and os.environ.get("FG_VARIANT_DIR"):
-        # A/B harness for kernel-shape experiments (profiles/variants.sh): another build of the SAME library
+        # A/B harness for kernel-shape experiments: another build of the SAME library
         p = Path(os.environ["FG_VARIANT_DIR"]) / name
     if not p.exists():
         raise NativeLibraryMissing(
-            f"{p} is missing: run `python -m flowgger_b200.build` (nvcc, sm_100a). "
+            f"{p} is missing: run `python -m flowgger_b200.build` (nvcc, sm_90a). "
             "flowgger_b200 has no CPU fallback.")
     return C.CDLL(str(p), mode=C.RTLD_GLOBAL)
 

@@ -1,9 +1,9 @@
-/* flowgger_cuda.h — C ABI of the B200 batched log-line decoder.
+/* flowgger_cuda.h — C ABI of the H100 batched log-line decoder.
  *
  * Drop-in boundary for flowgger's Decoder stage.  The reference interface this
  * replaces is
  *     trait Decoder { fn decode(&self, line: &str) -> Result<Record, &'static str>; }
- *         (/root/reference/src/flowgger/decoder/mod.rs:44-46)
+ *         (flowgger src/flowgger/decoder/mod.rs:44-46)
  * constructed by RFC5424Decoder::new / LTSVDecoder::new / GelfDecoder::new / RFC3164Decoder::new
  *         (decoder/rfc5424_decoder.rs:12, ltsv_decoder.rs:24, gelf_decoder.rs:16, rfc3164_decoder.rs:14)
  * and called once per record by the splitters
@@ -15,7 +15,7 @@
  * RFC5424 SD values are unescaped on the device into a small arena).
  *
  * Plain C: pointers and sizes only.  No CPU fallback exists behind this ABI:
- * every entry point that parses runs the sm_100a CUDA kernels or fails.
+ * every entry point that parses runs the sm_90a CUDA kernels or fails.
  */
 #ifndef FLOWGGER_CUDA_H
 #define FLOWGGER_CUDA_H

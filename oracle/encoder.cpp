@@ -2,7 +2,7 @@
 //
 // CPU restatement of the reference's GELF encoder, the stage that follows Decoder::decode in every splitter
 // (splitter/line_splitter.rs:50-52):
-//     GelfEncoder::encode      /root/reference/src/flowgger/encoder/gelf_encoder.rs:59-115
+//     GelfEncoder::encode      flowgger src/flowgger/encoder/gelf_encoder.rs:59-115
 //     GelfEncoder::new         gelf_encoder.rs:29-48 (output.gelf_extra)
 // The JSON text comes from un-vendored crates pinned in Cargo.toml: serde_json "~0.8" (`to_vec` over
 // Value::Object(BTreeMap<String, Value>): keys in byte order, last insert wins, compact separators) and its float

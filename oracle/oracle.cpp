@@ -2,7 +2,7 @@
 //
 // Line-by-line CPU restatement of the reference decoders.  Every function
 // cites the reference lines it follows (paths relative to
-// /root/reference/src/flowgger/).  Like the reference it builds an owned
+// flowgger src/flowgger/).  Like the reference it builds an owned
 // Record (one heap string per field) so that it is also a fair CPU baseline.
 #include "oracle.hpp"
 

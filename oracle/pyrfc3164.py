@@ -1,5 +1,5 @@
 """oracle/pyrfc3164.py — TEST INFRASTRUCTURE: a second, independent restatement of RFC3164Decoder::decode
-(/root/reference/src/flowgger/decoder/rfc3164_decoder.rs:31-213) in plain Python.
+(flowgger src/flowgger/decoder/rfc3164_decoder.rs:31-213) in plain Python.
 
 It shares no code with oracle/rfc3164.cpp or with the product: tokens come from a regular expression over Rust's
 White_Space set, dates from `datetime`, zones from the standard library's `zoneinfo` (fold = 0) instead of the TZif readers

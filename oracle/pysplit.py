@@ -1,5 +1,5 @@
 """oracle/pysplit.py — TEST INFRASTRUCTURE: CPU restatement of the framing LineSplitter::run performs before decode
-(/root/reference/src/flowgger/splitter/line_splitter.rs:17-25): `BufRead::lines` (split at b'\\n', drop it and ONE
+(flowgger src/flowgger/splitter/line_splitter.rs:17-25): `BufRead::lines` (split at b'\\n', drop it and ONE
 preceding b'\\r'; an unterminated last line is still yielded; an empty stream yields nothing) and the UTF-8 check of
 `String` (invalid => the line is skipped with "Invalid UTF-8 input")."""
 from __future__ import annotations
@@ -34,7 +34,7 @@ def split_lines(stream: bytes) -> tuple[np.ndarray, list[bytes], list[bool]]:
 
 
 def split_nul(stream: bytes) -> tuple[np.ndarray, list[bytes], list[bool]]:
-    """NulSplitter::run (/root/reference/src/flowgger/splitter/nul_splitter.rs:18-40): `BufRead::split(0)` — records end at
+    """NulSplitter::run (flowgger src/flowgger/splitter/nul_splitter.rs:18-40): `BufRead::split(0)` — records end at
     a NUL byte, which is dropped; nothing else is stripped; an unterminated last record is still yielded; invalid UTF-8 =>
     "Invalid UTF-8 input" and the record is skipped.  Same return shape as split_lines."""
     if len(stream) == 0:

@@ -1,6 +1,6 @@
 // oracle/rfc3164.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE (see oracle.hpp).
 //
-// CPU restatement of RFC3164Decoder::decode (/root/reference/src/flowgger/decoder/rfc3164_decoder.rs:31-213), written
+// CPU restatement of RFC3164Decoder::decode (flowgger src/flowgger/decoder/rfc3164_decoder.rs:31-213), written
 // the way the reference is: owned token vectors, the "standard" form first, the "custom" form second.
 //
 // Un-vendored crates on this path, restated from their published behaviour:

@@ -1,4 +1,4 @@
-//! cuda_decoder — `flowgger::decoder::Decoder` implementations backed by the B200 batched parser.
+//! cuda_decoder — `flowgger::decoder::Decoder` implementations backed by the H100 batched parser.
 //!
 //! Mirrors flowgger_b200/csrc/host/flowgger.{hpp,cpp} (the C++ twin that the test-suite drives, because the
 //! build environment has no Rust toolchain).  Reference interfaces implemented here:

@@ -11,7 +11,7 @@ sys.path.insert(0, str(REPO / "oracle"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _cuda_devices() -> int:

@@ -45,19 +45,17 @@ def test_error_strings_match_reference_text(native):
 
 
 def test_reference_strings_present_in_reference_sources():
-    """Guard against typos: each error string must occur verbatim in the reference decoder sources
-    (only checked where /root/reference exists, i.e. in the build container)."""
-    ref = Path("/root/reference/src/flowgger/decoder")
-    if not ref.exists():
-        return
+    """Guard against typos: each error string must occur verbatim in a string literal of the reference decoder and
+    line-splitter sources (stored in tests/golden/reference_strings.json)."""
+    import json
     import flowgger_b200 as fb
-    src = "".join(p.read_text() for p in ref.glob("*_decoder.rs"))
-    src += Path("/root/reference/src/flowgger/splitter/line_splitter.rs").read_text()  # "Invalid UTF-8 input"
-    src_flat = re.sub(r'"\s*\\\n\s*', "", src)
+    golden = json.loads((REPO / "tests" / "golden" / "reference_strings.json").read_text())["literals"]
+    assert "src/flowgger/splitter/line_splitter.rs" in golden  # "Invalid UTF-8 input"
+    literals = [s for per_file in golden.values() for s in per_file]
     for s in range(1, fb.load_cuda().fg_error_count()):
         e = fb.error_string(0, s)
         if e and not e.startswith("(the reference panics here"):  # FG_E3_PANIC is this repo's name for a reference panic
-            assert e in src_flat, e
+            assert any(e in lit for lit in literals), e
 
 
 def test_no_cpu_fallback_without_gpu(native):
@@ -70,8 +68,19 @@ def test_no_cpu_fallback_without_gpu(native):
         native.BatchDecoder(native.FMT_RFC5424)
 
 
-def test_build_info_names_sm100a(native):
-    assert "sm_100a" in native.build_info()
+def test_build_info_names_sm90a(native):
+    """The build string names sm_90a, and every device image embedded in the library is an sm_90a cubin (no other
+    architecture, no PTX to JIT)."""
+    import subprocess
+    from flowgger_b200 import build as fb_build
+    assert "sm_90a" in native.build_info()
+    cuobjdump = str(Path(fb_build.NVCC).parent / "cuobjdump")
+    lib = str(native.cuda_lib_path())
+    elves = re.findall(r"\.(sm_\w+)\.cubin", subprocess.run([cuobjdump, "--list-elf", lib], capture_output=True, text=True,
+                                                            check=True).stdout)
+    assert elves and set(elves) == {"sm_90a"}, elves
+    ptx = subprocess.run([cuobjdump, "--list-ptx", lib], capture_output=True, text=True, check=True).stdout
+    assert "PTX file" not in ptx, ptx
 
 
 def test_generator_is_deterministic(native):

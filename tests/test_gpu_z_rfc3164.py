@@ -1,6 +1,5 @@
 """RFC3164 on the device (SURVEY.md §8(f) N3): parse3164_kernel through the C ABI against the oracle.
-(The file sorts last on purpose: the format was added in the last session of round 2, with 5.5 GPU-minutes left; these tests
-passed on the B200 with the shipped build, profiles/r2s_pytest_rfc3164_lockstep.log, DESIGN.md §10.)"""
+(The file sorts last on purpose: the format was added last, so the older formats' GPU tests run first.)"""
 import numpy as np
 import pytest
 
