@@ -87,8 +87,103 @@ struct ErrorTableInit {
 constexpr size_t kPad = 256;            // slack after the device byte buffer (16-byte bulk-copy granules)
 constexpr size_t kBounceBytes = 32u << 20;  // pinned bounce buffers for pageable caller memory
 constexpr size_t kL2FlushBytes = 256u << 20;
-constexpr int kCnt = 8;                 // u32 counters snapshotted per chunk (fg::K5_* + the bad-offsets flag)
-constexpr int kBadFlag = 6;             // d_k[kBadFlag]: set by check_offsets_kernel
+constexpr size_t kCountBytes = sizeof(uint32_t) * fg::K5_COUNT;  // one snapshot of the counter block
+
+enum Where { DEV = 1, HOST = 2, BOTH = 3 };
+
+// A device array, a pinned host array, or both of the same length (the host one mirrors the device one); freed when
+// it is dropped or reallocated.
+template <class T, class H = T>
+struct Buf {
+    static_assert(sizeof(T) == sizeof(H), "the pinned mirror has the layout of the device array");
+    T* d = nullptr;
+    H* h = nullptr;
+    size_t n = 0;  // elements, once allocated
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { reset(); }
+    void reset() {
+        if (d) cudaFree(d);
+        if (h) cudaFreeHost(h);
+        d = nullptr;
+        h = nullptr;
+        n = 0;
+    }
+    cudaError_t alloc(size_t count, Where w) {
+        reset();
+        cudaError_t e = (w & DEV) ? cudaMalloc((void**)&d, count * sizeof(T)) : cudaSuccess;
+        if (e == cudaSuccess && (w & HOST)) e = cudaHostAlloc((void**)&h, count * sizeof(H), cudaHostAllocDefault);
+        if (e == cudaSuccess) n = count;
+        return e;
+    }
+};
+
+void destroy(cudaEvent_t e) { cudaEventDestroy(e); }
+void destroy(cudaStream_t s) { cudaStreamDestroy(s); }
+// An owned event or stream
+template <class H>
+struct Handle {
+    H h = nullptr;
+    Handle() = default;
+    Handle(Handle&& o) noexcept : h(o.h) { o.h = nullptr; }
+    Handle(const Handle&) = delete;
+    Handle& operator=(const Handle&) = delete;
+    ~Handle() {
+        if (h) destroy(h);
+    }
+    operator H() const { return h; }
+};
+using Event = Handle<cudaEvent_t>;
+using Stream = Handle<cudaStream_t>;
+
+// the events of one parse step of a pipelined call
+struct StepEvents {
+    Event h2d;     // its input is on the device
+    Event k0, k1;  // bracket its kernels
+    Event cnt;     // its counter snapshot is on the host
+};
+
+// Side tables: the kernels bump-allocate their rows through a word of the counter block, which keeps counting past the
+// capacity when a batch does not fit; the batch is then redone after a regrow to the reported need.  A table is up to
+// three columns (device array + pinned mirror) of `width` bytes per row that share one capacity.
+enum { T_ENTRIES, T_E8, T_ARENA, T_WIDE, T_COUNT };
+struct TableShape {
+    size_t width[3];
+    size_t round;  // rows are allocated in multiples of this
+};
+constexpr TableShape kTableShape[T_COUNT] = {
+    {{sizeof(fg_span), sizeof(uint64_t), 1}, 256},  // T_ENTRIES: 17-byte rows (LTSV, GELF, RFC5424 wide lines)
+    {{sizeof(uint64_t), 0, 0}, 256},                // T_E8: RFC5424 8-byte entries
+    {{1, 0, 0}, 256},                               // T_ARENA: RFC5424 unescaped values, RFC3164 re-joined messages
+    {{sizeof(fg_wide_row), 0, 0}, 1},               // T_WIDE: RFC5424 wide rows
+};
+static_assert(sizeof(fg_span) == sizeof(int2) && sizeof(fg_wide_row) == sizeof(fg::WideRow), "pinned rows mirror the device rows");
+struct Table {
+    Buf<uint8_t> col[3];
+    size_t cap = 0;  // rows
+};
+
+// The tables a format uses, the counter that fills each (-1: none, the table stays empty) and its size on first use,
+// max(max_bytes / div, floor) rows (`grow`: also whenever it is smaller than that)
+struct TableUse {
+    int table, counter;
+    size_t div, floor;
+    bool grow;
+};
+struct FormatTables {
+    int n;
+    TableUse use[4];
+    const TableUse* begin() const { return use; }
+    const TableUse* end() const { return use + n; }
+};
+constexpr FormatTables kFormatTables[4] = {
+    {4, {{T_E8, fg::K5_ENTRIES, 24, 4096, false}, {T_ARENA, fg::K5_ARENA, 64, 64 << 10, false},
+         {T_WIDE, fg::K5_WIDE_ROWS, 0, 1024, false}, {T_ENTRIES, fg::K5_WIDE_ENTRIES, 0, 4096, false}}},  // RFC5424
+    {1, {{T_ENTRIES, fg::K5_ENTRIES, 24, 4096, true}}},                                                  // LTSV
+    {1, {{T_ENTRIES, fg::K5_ENTRIES, 24, 4096, true}}},                                                  // GELF
+    {2, {{T_ARENA, fg::K5_ARENA, 32, 64 << 10, false}, {T_ENTRIES, -1, 0, 256, false}}},                 // RFC3164
+};
 
 }  // namespace
 
@@ -97,101 +192,71 @@ struct fg_ctx {
     size_t max_bytes = 0;
     int max_lines = 0;
     int chunk_lines = 0;
-    cudaStream_t s_h2d = nullptr, s_comp = nullptr, s_d2h = nullptr;
+    Stream s_h2d, s_comp, s_d2h;
+    Stream s_parse;  // split mode: the parse kernels, behind the framing on s_comp
+    Event ev_a, ev_b;
+    Event ev_dom0, ev_dom1;  // bracket the dominant kernel of a resident step
+    Event ev_s0, ev_s1;      // bracket the framing of a split call
+    std::vector<StepEvents> steps;
+    std::vector<Event> ev_split;  // split mode: chunk k is framed and validated
+    Event bounce_ev[2];
+    Buf<uint8_t> bounce[2];   // pinned bounce buffers
+    Buf<uint32_t> counts;     // pinned per-step snapshots of the counter block (K5_COUNT words each)
     // device: input
-    uint8_t* d_bytes = nullptr;
-    int32_t* d_offsets = nullptr;
-    uint32_t* d_k = nullptr;  // counter block (fg::K5_* ; [kBadFlag] = offsets check)
-    uint8_t* d_flush = nullptr;
-    // LTSV / GELF: columnar rows (9 columns sized for max_lines) + 17-byte side-table rows + scratch.
-    // The side-table arrays also hold the rows of the RFC5424 wide lines.
-    uint8_t* d_rows = nullptr;
-    uint8_t* h_rows = nullptr;
-    int2* d_entry_name = nullptr;
-    unsigned long long* d_entry_val = nullptr;
-    uint8_t* d_entry_meta = nullptr;
-    fg_span* h_entry_name = nullptr;
-    uint64_t* h_entry_val = nullptr;
-    uint8_t* h_entry_meta = nullptr;
-    size_t entry_cap = 0;
-    int2* d_tmp_name = nullptr;  // provisional side-table rows, indexed by byte offset / scratch_div
-    unsigned long long* d_tmp_val = nullptr;
-    uint8_t* d_tmp_meta = nullptr;
-    size_t tmp_cap = 0;
-    // RFC5424: compact rows, 8-byte entries, work lists, arena, wide rows
-    uint4* d_rows5 = nullptr;
-    fg_row5424* h_rows5 = nullptr;
-    unsigned long long* d_e8 = nullptr;
-    uint64_t* h_e8 = nullptr;
-    size_t e8_cap = 0;
-    uint32_t* d_esc_list = nullptr;
-    uint32_t* d_wide_list = nullptr;
-    uint8_t* d_arena = nullptr;
-    uint8_t* h_arena = nullptr;
-    size_t arena_cap = 0;
-    fg::WideRow* d_wide = nullptr;
-    fg_wide_row* h_wide = nullptr;
-    size_t wide_cap = 0;
+    Buf<uint8_t> bytes;
+    Buf<int32_t> offsets;
+    Buf<uint32_t> k;  // counter block (fg::K5_*)
+    Buf<uint8_t> flush;
+    // side tables
+    Table tab[T_COUNT];
+    // LTSV / GELF / RFC3164: columnar rows (9 columns sized for max_lines); LTSV / GELF: scratch side-table rows
+    Buf<uint8_t> rows;
+    Buf<int2> tmp_name;  // provisional side-table rows, indexed by byte offset / scratch_div
+    Buf<unsigned long long> tmp_val;
+    Buf<uint8_t> tmp_meta;
+    // RFC5424: compact rows, work lists (the wide list is also GELF's slow list)
+    Buf<fg::Row5424, fg_row5424> rows5;
+    Buf<uint32_t> esc_list, wide_list;
     // fused GELF encoder (fg_decode_encode_gelf)
-    uint32_t* d_enc_lens = nullptr;
-    uint32_t* d_enc_rel = nullptr;
-    unsigned long long* d_enc_base = nullptr;  // [chunks + 1] running output size
-    unsigned long long* h_enc_base = nullptr;
-    int enc_base_cap = 0;
-    uint8_t* d_enc_out = nullptr;
-    uint8_t* h_enc_out = nullptr;
-    size_t enc_out_cap = 0;
-    long long* d_enc_offsets = nullptr;
-    int64_t* h_enc_offsets = nullptr;
-    uint8_t* d_enc_status = nullptr;
-    uint8_t* h_enc_status = nullptr;
-    void* d_scan_temp = nullptr;
+    Buf<uint32_t> enc_lens, enc_rel;
+    Buf<unsigned long long> enc_base;  // [chunks + 1] running output size
+    Buf<uint8_t> enc_out;
+    size_t enc_out_cap = 0;  // enc_out holds 16 bytes more
+    Buf<long long, int64_t> enc_offsets;
+    Buf<uint8_t> enc_status;
+    Buf<uint8_t> scan_temp;
     size_t scan_temp_bytes = 0;
-    uint8_t* d_static_blob = nullptr;  // fixed GELF keys + output.gelf_extra, sorted
+    Buf<uint8_t> static_blob;  // fixed GELF keys + output.gelf_extra, sorted
     int n_static = 0;
     const int32_t* d_static_key_off = nullptr;
     const int32_t* d_static_lit_off = nullptr;
     const int32_t* d_static_kind = nullptr;
     std::vector<std::pair<std::string, std::string>> gelf_extra;
     // split mode (fg_split_decode)
-    uint32_t* d_seg = nullptr;
-    int32_t* d_n_lines = nullptr;
-    uint8_t* d_invalid = nullptr;
-    int32_t* h_offsets = nullptr;
-    int32_t* h_n_lines = nullptr;
+    Buf<uint32_t> seg;
+    Buf<int32_t> n_lines;
+    Buf<uint8_t> invalid;
+    Buf<int32_t> split_offsets;  // pinned: the line offsets found on the device
+    Buf<int32_t> cum;
     float last_split_ms = 0.f;
-    cudaEvent_t ev_s0 = nullptr, ev_s1 = nullptr;
-    cudaStream_t s_parse = nullptr;
-    std::vector<cudaEvent_t> ev_split;
-    int32_t* d_cum = nullptr;
-    int32_t* h_cum = nullptr;
     // RFC3164: the year `now_utc().year()` stands for (0: read the clock at every call) and the zone database
     int r3164_year = 0;
     int call_year = 1970;  // the year of the call in progress (current_year())
     std::string tzdir;
     fg::TzHostTable tz_host;
-    uint8_t* d_tz_blob = nullptr;
+    Buf<uint8_t> tz_blob;
     fg::TzDeviceTable tz_dev{};
-    // LTSV config blobs
-    uint8_t* d_ltsv_blob = nullptr;
+    // LTSV config blob
+    Buf<uint8_t> ltsv_blob;
     fg::LtsvDeviceConfig ltsv{};
-    // pinned host
-    uint32_t* h_counts = nullptr;  // per-chunk snapshots of the counter block (kCnt words each)
-    int h_counts_cap = 0;
-    uint8_t* h_bounce[2] = {nullptr, nullptr};
-    cudaEvent_t bounce_ev[2] = {nullptr, nullptr};
-    std::vector<cudaEvent_t> ev_h2d, ev_k0, ev_k1, ev_cnt;
-    cudaEvent_t ev_a = nullptr, ev_b = nullptr;
-    cudaEvent_t ev_dom0 = nullptr, ev_dom1 = nullptr;  // bracket the dominant kernel of a resident step
     float last_dom_ms = 0.f;
     // resident batch
     int res_n = 0;
     size_t res_bytes = 0;
     int res_fmt = -1;
-    uint32_t res_tot[kCnt] = {};
+    uint32_t res_tot[fg::K5_COUNT] = {};
     std::string last_error;
     int64_t launches = 0;
-    int max_tile = 0;   // LTSV / GELF staging tile limit
     int max_tile5 = 0;  // RFC5424: tile + bitmap must fit the opt-in shared memory
     int num_sms = 0;    // of the device: the post kernels' fixed grids stride over their work lists with a few CTAs per SM
 };
@@ -224,94 +289,132 @@ int fail(fg_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess) {
         if (_e != cudaSuccess) return fail(ctx, FG_E_CUDA, #call, _e); \
     } while (0)
 
+cudaError_t create(Event& e, unsigned flags) { return cudaEventCreateWithFlags(&e.h, flags); }
+cudaError_t create(Stream& s) { return cudaStreamCreateWithFlags(&s.h, cudaStreamNonBlocking); }
+
 template <class T>
-void dfree(T*& p) {
-    if (p) cudaFree(p);
-    p = nullptr;
+T* dev(const fg_ctx* c, int t, int col = 0) {
+    return reinterpret_cast<T*>(c->tab[t].col[col].d);
 }
 template <class T>
-void hfree(T*& p) {
-    if (p) cudaFreeHost(p);
-    p = nullptr;
+T* host(const fg_ctx* c, int t, int col = 0) {
+    return reinterpret_cast<T*>(c->tab[t].col[col].h);
+}
+uint32_t cap32(const fg_ctx* c, int t) { return (uint32_t)std::min<size_t>(c->tab[t].cap, 0xFFFFFFFFu); }
+
+// (re)allocates table t for `rows` rows; its old columns are all freed first
+int grow_table(fg_ctx* c, int t, size_t rows) {
+    const TableShape& S = kTableShape[t];
+    Table& T = c->tab[t];
+    T.cap = 0;
+    for (auto& col : T.col) col.reset();
+    rows = (rows + S.round - 1) / S.round * S.round;
+    for (int i = 0; i < 3 && S.width[i]; ++i) FG_CUDA(c, T.col[i].alloc(rows * S.width[i], BOTH));
+    T.cap = rows;
+    return FG_OK;
 }
 
-// 17-byte side-table rows (LTSV / GELF, RFC5424 wide lines)
-int alloc_entries(fg_ctx* c, size_t cap) {
-    dfree(c->d_entry_name); dfree(c->d_entry_val); dfree(c->d_entry_meta);
-    hfree(c->h_entry_name); hfree(c->h_entry_val); hfree(c->h_entry_meta);
-    c->entry_cap = 0;
-    cap = (cap + 255) & ~(size_t)255;
-    FG_CUDA(c, cudaMalloc(&c->d_entry_name, cap * sizeof(int2)));
-    FG_CUDA(c, cudaMalloc(&c->d_entry_val, cap * sizeof(unsigned long long)));
-    FG_CUDA(c, cudaMalloc(&c->d_entry_meta, cap));
-    FG_CUDA(c, cudaHostAlloc(&c->h_entry_name, cap * sizeof(fg_span), cudaHostAllocDefault));
-    FG_CUDA(c, cudaHostAlloc(&c->h_entry_val, cap * sizeof(uint64_t), cudaHostAllocDefault));
-    FG_CUDA(c, cudaHostAlloc(&c->h_entry_meta, cap, cudaHostAllocDefault));
-    c->entry_cap = cap;
+// tables whose fill level the kernels report in the counter block
+bool tables_overflow(const fg_ctx* c, int fmt, const uint32_t* t) {
+    for (const TableUse& u : kFormatTables[fmt])
+        if (u.counter >= 0 && t[u.counter] > c->tab[u.table].cap) return true;
+    return false;
+}
+int regrow_tables(fg_ctx* c, int fmt, const uint32_t* t) {
+    for (const TableUse& u : kFormatTables[fmt]) {
+        const size_t need = u.counter >= 0 ? t[u.counter] : 0;
+        if (need > c->tab[u.table].cap)
+            if (int rc = grow_table(c, u.table, need + need / 8 + 1024)) return rc;
+    }
     return FG_OK;
 }
-int alloc_e8(fg_ctx* c, size_t cap) {
-    dfree(c->d_e8); hfree(c->h_e8);
-    c->e8_cap = 0;
-    cap = (cap + 255) & ~(size_t)255;
-    FG_CUDA(c, cudaMalloc(&c->d_e8, cap * 8));
-    FG_CUDA(c, cudaHostAlloc(&c->h_e8, cap * 8, cudaHostAllocDefault));
-    c->e8_cap = cap;
+
+// side tables: the rows a chunk produced are the contiguous range [prev, cur) of each bump allocator
+int copy_tables_d2h(fg_ctx* c, int fmt, const uint32_t* prev, const uint32_t* cur, cudaStream_t s) {
+    for (const TableUse& u : kFormatTables[fmt]) {
+        if (u.counter < 0 || cur[u.counter] <= prev[u.counter]) continue;
+        const size_t from = prev[u.counter], rows = cur[u.counter] - prev[u.counter];
+        const TableShape& S = kTableShape[u.table];
+        const Table& T = c->tab[u.table];
+        for (int i = 0; i < 3 && S.width[i]; ++i)
+            FG_CUDA(c, cudaMemcpyAsync(T.col[i].h + from * S.width[i], T.col[i].d + from * S.width[i], rows * S.width[i],
+                                       cudaMemcpyDeviceToHost, s));
+    }
     return FG_OK;
 }
-int alloc_arena(fg_ctx* c, size_t cap) {
-    dfree(c->d_arena); hfree(c->h_arena);
-    c->arena_cap = 0;
-    cap = (cap + 255) & ~(size_t)255;
-    FG_CUDA(c, cudaMalloc(&c->d_arena, cap));
-    FG_CUDA(c, cudaHostAlloc(&c->h_arena, cap, cudaHostAllocDefault));
-    c->arena_cap = cap;
-    return FG_OK;
-}
-int alloc_wide(fg_ctx* c, size_t cap) {
-    dfree(c->d_wide); hfree(c->h_wide);
-    c->wide_cap = 0;
-    FG_CUDA(c, cudaMalloc(&c->d_wide, cap * sizeof(fg::WideRow)));
-    FG_CUDA(c, cudaHostAlloc(&c->h_wide, cap * sizeof(fg_wide_row), cudaHostAllocDefault));
-    c->wide_cap = cap;
-    return FG_OK;
-}
+
+// Host arrays placed at 16-byte aligned offsets of one device blob, uploaded at once.  A zeroed 16-byte tail follows
+// the last array: device code may read whole words past the end of an array.
+struct Packer {
+    std::vector<uint8_t> bytes;
+    template <class V>
+    size_t add(const V& v) {
+        const size_t at = bytes.size();
+        const uint8_t* src = reinterpret_cast<const uint8_t*>(v.data());
+        bytes.insert(bytes.end(), src, src + v.size() * sizeof(v[0]));
+        bytes.resize((bytes.size() + 15) & ~(size_t)15, 0);
+        return at;
+    }
+    int upload(fg_ctx* c, Buf<uint8_t>& blob) {
+        bytes.resize(bytes.size() + 16, 0);
+        FG_CUDA(c, blob.alloc(bytes.size(), DEV));
+        FG_CUDA(c, cudaMemcpy(blob.d, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
+        return FG_OK;
+    }
+};
 
 // packed zone table -> one device blob (fg::TzDeviceTable points into it)
 int upload_tz(fg_ctx* c) {
     const fg::TzHostTable& H = c->tz_host;
-    dfree(c->d_tz_blob);
-    size_t o = 0;
-    auto place = [&](size_t bytes) {
-        const size_t at = o;
-        o += (bytes + 15) & ~(size_t)15;
-        return at;
-    };
-    const size_t o_hash = place(H.hash.size() * 8), o_key = place(H.key.size() * 8), o_zone = place(H.zone.size() * 4),
-                 o_noff = place(H.name_off.size() * 4), o_first = place(H.first.size() * 4), o_off = place(H.off.size() * 4),
-                 o_names = place(H.names.size());
-    std::vector<uint8_t> blob(o + 16, 0);
-    auto put = [&](size_t at, const void* src, size_t bytes) {
-        if (bytes) memcpy(blob.data() + at, src, bytes);
-    };
-    put(o_hash, H.hash.data(), H.hash.size() * 8);
-    put(o_key, H.key.data(), H.key.size() * 8);
-    put(o_zone, H.zone.data(), H.zone.size() * 4);
-    put(o_noff, H.name_off.data(), H.name_off.size() * 4);
-    put(o_first, H.first.data(), H.first.size() * 4);
-    put(o_off, H.off.data(), H.off.size() * 4);
-    put(o_names, H.names.data(), H.names.size());
-    FG_CUDA(c, cudaMalloc(&c->d_tz_blob, blob.size()));
-    FG_CUDA(c, cudaMemcpy(c->d_tz_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice));
+    Packer p;
+    const size_t o_hash = p.add(H.hash), o_key = p.add(H.key), o_zone = p.add(H.zone), o_noff = p.add(H.name_off),
+                 o_first = p.add(H.first), o_off = p.add(H.off), o_names = p.add(H.names);
+    if (int rc = p.upload(c, c->tz_blob)) return rc;
+    const uint8_t* b = c->tz_blob.d;
     fg::TzDeviceTable& T = c->tz_dev;
     T = H.view();
-    T.hash = (const unsigned long long*)(c->d_tz_blob + o_hash);
-    T.key = (const long long*)(c->d_tz_blob + o_key);
-    T.zone = (const int32_t*)(c->d_tz_blob + o_zone);
-    T.name_off = (const int32_t*)(c->d_tz_blob + o_noff);
-    T.first = (const int32_t*)(c->d_tz_blob + o_first);
-    T.off = (const int32_t*)(c->d_tz_blob + o_off);
-    T.names = c->d_tz_blob + o_names;
+    T.hash = (const unsigned long long*)(b + o_hash);
+    T.key = (const long long*)(b + o_key);
+    T.zone = (const int32_t*)(b + o_zone);
+    T.name_off = (const int32_t*)(b + o_noff);
+    T.first = (const int32_t*)(b + o_first);
+    T.off = (const int32_t*)(b + o_off);
+    T.names = b + o_names;
+    return FG_OK;
+}
+
+// LTSV schema / suffixes -> one device blob
+int upload_ltsv_config(fg_ctx* c, const fg_config* cfg) {
+    std::vector<uint8_t> names, suffix;
+    std::vector<int32_t> name_off{0}, types;
+    const int ns = (cfg->ltsv_schema_names && cfg->ltsv_schema_types) ? cfg->ltsv_schema_len : 0;
+    for (int k = 0; k < ns; ++k) {
+        const char* s = cfg->ltsv_schema_names[k];
+        names.insert(names.end(), (const uint8_t*)s, (const uint8_t*)s + strlen(s));
+        name_off.push_back((int32_t)names.size());
+        types.push_back(cfg->ltsv_schema_types[k]);
+    }
+    fg::LtsvDeviceConfig& L = c->ltsv;
+    L.has_schema = (cfg->ltsv_has_schema || ns > 0) ? 1 : 0;
+    L.n_schema = ns;
+    L.suffix_present = 0;
+    L.suffix_off[0] = 0;
+    for (int t = 0; t < 5; ++t) {
+        const char* s = cfg->ltsv_suffix[t];
+        if (t > 0 && s) {
+            L.suffix_present |= 1u << t;
+            suffix.insert(suffix.end(), (const uint8_t*)s, (const uint8_t*)s + strlen(s));
+        }
+        L.suffix_off[t + 1] = (int32_t)suffix.size();
+    }
+    Packer p;
+    const size_t o_names = p.add(names), o_off = p.add(name_off), o_types = p.add(types), o_suf = p.add(suffix);
+    if (int rc = p.upload(c, c->ltsv_blob)) return rc;
+    const uint8_t* b = c->ltsv_blob.d;
+    L.names = b + o_names;
+    L.name_off = (const int32_t*)(b + o_off);
+    L.types = (const int32_t*)(b + o_types);
+    L.suffix = b + o_suf;
     return FG_OK;
 }
 
@@ -326,96 +429,64 @@ int current_year(const fg_ctx* c) {
 
 // Format-specific buffers are allocated on first use of the format.
 int ensure_format(fg_ctx* c, int fmt) {
+    const size_t L = (size_t)c->max_lines;
     if (fmt == FG_FMT_RFC5424) {
-        if (!c->d_rows5) {
-            FG_CUDA(c, cudaMalloc(&c->d_rows5, (size_t)c->max_lines * 32));
-            FG_CUDA(c, cudaHostAlloc(&c->h_rows5, (size_t)c->max_lines * 32, cudaHostAllocDefault));
-            FG_CUDA(c, cudaMalloc(&c->d_esc_list, (size_t)c->max_lines * 4));
-            FG_CUDA(c, cudaMalloc(&c->d_wide_list, (size_t)c->max_lines * 4));
+        if (!c->rows5.d) {
+            FG_CUDA(c, c->rows5.alloc(L, BOTH));
+            FG_CUDA(c, c->esc_list.alloc(L, DEV));
+            FG_CUDA(c, c->wide_list.alloc(L, DEV));
         }
-        if (!c->e8_cap)
-            if (int rc = alloc_e8(c, std::max<size_t>(c->max_bytes / 24, 4096))) return rc;
-        if (!c->arena_cap)
-            if (int rc = alloc_arena(c, std::max<size_t>(c->max_bytes / 64, 64 << 10))) return rc;
-        if (!c->wide_cap)
-            if (int rc = alloc_wide(c, 1024)) return rc;
-        if (!c->entry_cap)
-            if (int rc = alloc_entries(c, 4096)) return rc;
-        return FG_OK;
+    } else if (!c->rows.d) {
+        FG_CUDA(c, c->rows.alloc(col_off(c, C_COUNT), BOTH));
     }
-    if (!c->d_rows) {
-        const size_t rows_bytes = col_off(c, C_COUNT);
-        FG_CUDA(c, cudaMalloc(&c->d_rows, rows_bytes));
-        FG_CUDA(c, cudaHostAlloc(&c->h_rows, rows_bytes, cudaHostAllocDefault));
+    if (fmt == FG_FMT_GELF && !c->wide_list.d) FG_CUDA(c, c->wide_list.alloc(L, DEV));  // slow list
+    for (const TableUse& u : kFormatTables[fmt]) {
+        const size_t first = u.div ? std::max<size_t>(c->max_bytes / u.div, u.floor) : u.floor;
+        const size_t cap = c->tab[u.table].cap;
+        if (u.grow ? cap < first : !cap)
+            if (int rc = grow_table(c, u.table, first)) return rc;
     }
-    if (fmt == FG_FMT_RFC3164) {  // no side table; re-joined messages go to the arena; zone names need the database
-        if (!c->arena_cap)
-            if (int rc = alloc_arena(c, std::max<size_t>(c->max_bytes / 32, 64 << 10))) return rc;
-        if (!c->entry_cap)
-            if (int rc = alloc_entries(c, 256)) return rc;
+    if (fmt == FG_FMT_RFC3164) {  // zone names need the database
         if (!c->tz_host.loaded) {
             std::string err;
             if (!fg::tz_load_dir(c->tzdir.empty() ? nullptr : c->tzdir.c_str(), c->tz_host, err)) return fail(c, FG_E_ARG, err.c_str());
         }
-        if (!c->d_tz_blob)
+        if (!c->tz_blob.d)
             if (int rc = upload_tz(c)) return rc;
-        return FG_OK;
     }
-    if (fmt == FG_FMT_GELF && !c->d_wide_list) FG_CUDA(c, cudaMalloc(&c->d_wide_list, (size_t)c->max_lines * 4));  // slow list
-    const size_t want = std::max<size_t>(c->max_bytes / 24, 4096);
-    if (c->entry_cap < want)
-        if (int rc = alloc_entries(c, want)) return rc;
-    // Scratch table for provisional side-table rows, indexed by byte offset (see Format<>::scratch_index):
-    // a row needs >= 3 input bytes in GELF, >= 1 byte + its TAB in LTSV.
-    const size_t need = (fmt == FG_FMT_LTSV ? c->max_bytes / 2 + (size_t)c->max_lines : c->max_bytes / 3) + 64;
-    if (c->tmp_cap < need) {
-        dfree(c->d_tmp_name); dfree(c->d_tmp_val); dfree(c->d_tmp_meta);
-        c->tmp_cap = 0;
-        FG_CUDA(c, cudaMalloc(&c->d_tmp_name, need * sizeof(int2)));
-        FG_CUDA(c, cudaMalloc(&c->d_tmp_val, need * sizeof(unsigned long long)));
-        FG_CUDA(c, cudaMalloc(&c->d_tmp_meta, need));
-        c->tmp_cap = need;
+    if (fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF) {
+        // Scratch table for provisional side-table rows, indexed by byte offset (see Format<>::scratch_index):
+        // a row needs >= 3 input bytes in GELF, >= 1 byte + its TAB in LTSV.
+        const size_t need = (fmt == FG_FMT_LTSV ? c->max_bytes / 2 + L : c->max_bytes / 3) + 64;
+        if (c->tmp_meta.n < need) {  // allocated last: set once all three exist
+            c->tmp_name.reset(); c->tmp_val.reset(); c->tmp_meta.reset();
+            FG_CUDA(c, c->tmp_name.alloc(need, DEV));
+            FG_CUDA(c, c->tmp_val.alloc(need, DEV));
+            FG_CUDA(c, c->tmp_meta.alloc(need, DEV));
+        }
     }
     return FG_OK;
 }
 
-// shared-memory tile: mean span of a CTA's lines plus slack; the kernel handles whatever does not fit in extra rounds
+// validate the format, then the context's device, the format's buffers and the year of this call
+int begin_call(fg_ctx* c, fg_format fmt) {
+    if ((int)fmt < 0 || (int)fmt > 3) return fail(c, FG_E_ARG, "unknown format");
+    FG_CUDA(c, cudaSetDevice(c->device));
+    if (int rc = ensure_format(c, (int)fmt)) return rc;
+    c->call_year = current_year(c);
+    return FG_OK;
+}
+
+// shared-memory tile: mean span of a CTA's lines plus 2 % slack; the kernel handles whatever does not fit in extra rounds
 int pick_tile(const fg_ctx* c, size_t total_bytes, int n, int fmt) {
     const double mean = n > 0 ? (double)total_bytes / n : 0.0;
     const long lines = fg::lines_per_cta(fmt), gran = 8 * lines;  // 1 KiB steps for 128-line CTAs, 512 B for 64
-#ifndef FG_TILE_SLACK_PCT  // head room of the tile over the mean span of a CTA's lines (-DFG_TILE_SLACK_PCT=... tries others)
-#define FG_TILE_SLACK_PCT 102
-#endif
-    long t = (long)(mean * lines * (FG_TILE_SLACK_PCT / 100.0)) + gran;
+    const int max_tile[4] = {c->max_tile5, fg::kLtsvMaxTile, fg::kGelfMaxTile, fg::kR3164MaxTile};
+    long t = (long)(mean * lines * 1.02) + gran;
     t = (t + gran - 1) / gran * gran;
     t = std::max(t, 8L * 1024);
-    t = std::min(t, (long)(fmt == FG_FMT_RFC5424 ? c->max_tile5 : (fmt == FG_FMT_LTSV ? fg::kLtsvMaxTile : (fmt == FG_FMT_GELF ? fg::kGelfMaxTile : fg::kR3164MaxTile))));
+    t = std::min(t, (long)max_tile[fmt]);
     return (int)t;
-}
-
-// tables whose fill level the kernels report in the counter block
-bool tables_overflow(const fg_ctx* c, int fmt, const uint32_t* t) {
-    if (fmt == FG_FMT_RFC5424)
-        return t[fg::K5_ENTRIES] > c->e8_cap || t[fg::K5_ARENA] > c->arena_cap || t[fg::K5_WIDE_ROWS] > c->wide_cap ||
-               t[fg::K5_WIDE_ENTRIES] > c->entry_cap;
-    if (fmt == FG_FMT_RFC3164) return t[fg::K5_ARENA] > c->arena_cap;
-    return t[fg::K5_ENTRIES] > c->entry_cap;
-}
-int regrow_tables(fg_ctx* c, int fmt, const uint32_t* t) {
-    auto grown = [](size_t need) { return need + need / 8 + 1024; };
-    if (fmt == FG_FMT_RFC5424) {
-        if (t[fg::K5_ENTRIES] > c->e8_cap)
-            if (int rc = alloc_e8(c, grown(t[fg::K5_ENTRIES]))) return rc;
-        if (t[fg::K5_ARENA] > c->arena_cap)
-            if (int rc = alloc_arena(c, grown(t[fg::K5_ARENA]))) return rc;
-        if (t[fg::K5_WIDE_ROWS] > c->wide_cap)
-            if (int rc = alloc_wide(c, grown(t[fg::K5_WIDE_ROWS]))) return rc;
-        if (t[fg::K5_WIDE_ENTRIES] > c->entry_cap)
-            if (int rc = alloc_entries(c, grown(t[fg::K5_WIDE_ENTRIES]))) return rc;
-        return FG_OK;
-    }
-    if (fmt == FG_FMT_RFC3164) return alloc_arena(c, grown(t[fg::K5_ARENA]));
-    return alloc_entries(c, grown(t[fg::K5_ENTRIES]));
 }
 
 // One parse launch over lines [line0, line0 + n) of the resident offsets (for RFC5424: parse + unescape + wide kernels)
@@ -423,42 +494,42 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
                  bool time_dominant = false) {
     if (fmt == FG_FMT_RFC5424) {
         fg::Parse5424Params P;
-        P.bytes = c->d_bytes;
-        P.offsets = c->d_offsets + line0;
+        P.bytes = c->bytes.d;
+        P.offsets = c->offsets.d + line0;
         P.n = n;
         P.tile_bytes = tile;
-        P.rows = c->d_rows5 + 2 * (size_t)line0;
-        P.entries = c->d_e8;
-        P.entry_cap = (uint32_t)std::min<size_t>(c->e8_cap, 0xFFFFFFFFu);
-        P.counters = c->d_k;
-        P.esc_list = c->d_esc_list;
-        P.wide_list = c->d_wide_list;
-        P.arena = c->d_arena;
-        P.arena_cap = (uint32_t)std::min<size_t>(c->arena_cap, 0xFFFFFFFFu);
-        P.wide_rows = c->d_wide;
-        P.wide_cap = (uint32_t)c->wide_cap;
-        P.wentry_name = c->d_entry_name;
-        P.wentry_val = c->d_entry_val;
-        P.wentry_meta = c->d_entry_meta;
-        P.wentry_cap = (uint32_t)std::min<size_t>(c->entry_cap, 0xFFFFFFFFu);
+        P.rows = reinterpret_cast<uint4*>(c->rows5.d + line0);
+        P.entries = dev<unsigned long long>(c, T_E8);
+        P.entry_cap = cap32(c, T_E8);
+        P.counters = c->k.d;
+        P.esc_list = c->esc_list.d;
+        P.wide_list = c->wide_list.d;
+        P.arena = dev<uint8_t>(c, T_ARENA);
+        P.arena_cap = cap32(c, T_ARENA);
+        P.wide_rows = dev<fg::WideRow>(c, T_WIDE);
+        P.wide_cap = cap32(c, T_WIDE);
+        P.wentry_name = dev<int2>(c, T_ENTRIES, 0);
+        P.wentry_val = dev<unsigned long long>(c, T_ENTRIES, 1);
+        P.wentry_meta = dev<uint8_t>(c, T_ENTRIES, 2);
+        P.wentry_cap = cap32(c, T_ENTRIES);
         P.line0 = line0;
-        P.bad_offsets = c->d_k + kBadFlag;
+        P.bad_offsets = c->k.d + fg::K5_BAD_OFFSETS;
         P.line_invalid = invalid;
         P.strip_eol = strip_eol;
         P.num_sms = c->num_sms;
-        FG_CUDA(c, cudaMemsetAsync(c->d_k + fg::K5_ESC_LIST, 0, 8, s));  // the two work lists are per launch
-        FG_CUDA(c, fg::launch_parse5424(P, s, time_dominant ? c->ev_dom0 : nullptr, time_dominant ? c->ev_dom1 : nullptr));
+        FG_CUDA(c, cudaMemsetAsync(c->k.d + fg::K5_ESC_LIST, 0, 8, s));  // the two work lists are per launch
+        FG_CUDA(c, fg::launch_parse5424(P, s, time_dominant ? c->ev_dom0.h : nullptr, time_dominant ? c->ev_dom1.h : nullptr));
         c->launches += 2;  // parse5424_kernel + post5424_kernel
         return FG_OK;
     }
     fg::ParseParams P;
-    P.bytes = c->d_bytes;
-    P.offsets = c->d_offsets + line0;
+    P.bytes = c->bytes.d;
+    P.offsets = c->offsets.d + line0;
     P.n = n;
     P.line0 = line0;
     P.tile_bytes = tile;
     P.num_sms = c->num_sms;
-    uint8_t* r = c->d_rows;
+    uint8_t* r = c->rows.d;
     P.ts = (double*)(r + col_off(c, C_TS)) + line0;
     P.meta = (uint32_t*)(r + col_off(c, C_META)) + line0;
     P.host = (int2*)(r + col_off(c, C_HOST)) + line0;
@@ -468,26 +539,26 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
     P.msg = (int2*)(r + col_off(c, C_MSG)) + line0;
     P.full = (int2*)(r + col_off(c, C_FULL)) + line0;
     P.sd = (int2*)(r + col_off(c, C_SD)) + line0;
-    P.entry_name = c->d_entry_name;
-    P.entry_val = c->d_entry_val;
-    P.entry_meta = c->d_entry_meta;
-    P.tmp_name = c->d_tmp_name;
-    P.tmp_val = c->d_tmp_val;
-    P.tmp_meta = c->d_tmp_meta;
+    P.entry_name = dev<int2>(c, T_ENTRIES, 0);
+    P.entry_val = dev<unsigned long long>(c, T_ENTRIES, 1);
+    P.entry_meta = dev<uint8_t>(c, T_ENTRIES, 2);
+    P.tmp_name = c->tmp_name.d;
+    P.tmp_val = c->tmp_val.d;
+    P.tmp_meta = c->tmp_meta.d;
     P.line_invalid = invalid;
     P.strip_eol = strip_eol;
-    P.entry_counter = c->d_k + fg::K5_ENTRIES;
-    P.entry_cap = (uint32_t)std::min<size_t>(c->entry_cap, 0xFFFFFFFFu);
-    P.bad_offsets = c->d_k + kBadFlag;
-    P.slow_list = c->d_wide_list;
-    P.slow_count = c->d_k + fg::K5_WIDE_LIST;
-    if (fmt == FG_FMT_GELF) FG_CUDA(c, cudaMemsetAsync(c->d_k + fg::K5_WIDE_LIST, 0, 4, s));  // the work list is per launch
+    P.entry_counter = c->k.d + fg::K5_ENTRIES;
+    P.entry_cap = cap32(c, T_ENTRIES);
+    P.bad_offsets = c->k.d + fg::K5_BAD_OFFSETS;
+    P.slow_list = c->wide_list.d;
+    P.slow_count = c->k.d + fg::K5_WIDE_LIST;
+    if (fmt == FG_FMT_GELF) FG_CUDA(c, cudaMemsetAsync(c->k.d + fg::K5_WIDE_LIST, 0, 4, s));  // the work list is per launch
     P.ltsv = c->ltsv;
     P.r3164.year = c->call_year;
     P.r3164.tz = c->tz_dev;
-    P.r3164.arena = c->d_arena;
-    P.r3164.arena_cap = (uint32_t)std::min<size_t>(c->arena_cap, 0xFFFFFFFFu);
-    P.r3164.arena_counter = c->d_k + fg::K5_ARENA;
+    P.r3164.arena = dev<uint8_t>(c, T_ARENA);
+    P.r3164.arena_cap = cap32(c, T_ARENA);
+    P.r3164.arena_counter = c->k.d + fg::K5_ARENA;
     if (time_dominant) FG_CUDA(c, cudaEventRecord(c->ev_dom0, s));
     FG_CUDA(c, fg::launch_parse(fmt, P, s));
     if (time_dominant) FG_CUDA(c, cudaEventRecord(c->ev_dom1, s));
@@ -495,31 +566,73 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
     return FG_OK;
 }
 
+// The fused GELF encoder over the RFC5424 results of lines [l0, l0 + n), parse step k
+int launch_encode(fg_ctx* c, int k, int l0, int n, int tile, cudaStream_t s) {
+    fg::GelfEncodeParams E;
+    E.bytes = c->bytes.d;
+    E.offsets = c->offsets.d + l0;
+    E.n = n;
+    E.rows = reinterpret_cast<const uint4*>(c->rows5.d + l0);
+    E.entries = dev<unsigned long long>(c, T_E8);
+    E.arena = dev<uint8_t>(c, T_ARENA);
+    E.wide_rows = dev<fg::WideRow>(c, T_WIDE);
+    E.wentry_name = dev<int2>(c, T_ENTRIES, 0);
+    E.wentry_val = dev<unsigned long long>(c, T_ENTRIES, 1);
+    E.wentry_meta = dev<uint8_t>(c, T_ENTRIES, 2);
+    E.static_blob = c->static_blob.d;
+    E.n_static = c->n_static;
+    E.static_key_off = c->d_static_key_off;
+    E.static_lit_off = c->d_static_lit_off;
+    E.static_kind = c->d_static_kind;
+    E.lens = c->enc_lens.d + l0;
+    E.rel = c->enc_rel.d + l0;
+    E.base = c->enc_base.d + k;
+    E.out = c->enc_out.d;
+    E.out_cap = c->enc_out_cap;
+    E.out_offsets = c->enc_offsets.d + l0;
+    E.status = c->enc_status.d + l0;
+    E.bad_offsets = c->k.d + fg::K5_BAD_OFFSETS;
+    E.entry_cap = cap32(c, T_E8);
+    E.wide_cap = cap32(c, T_WIDE);
+    E.wentry_cap = cap32(c, T_ENTRIES);
+    E.tile_bytes = std::min(4 * tile, c->max_tile5);  // the encoder's CTAs take 256 lines (4 x the parse kernel's 64)
+    FG_CUDA(c, fg::launch_gelf_encode(E, c->scan_temp.d, c->scan_temp_bytes, s));
+    c->launches += 4;
+    return FG_OK;
+}
+
 bool col_used(int col) { return !(col == C_APP || col == C_PROC || col == C_MSGID); }  // LTSV / GELF have no such fields
 
 void fill_out(fg_ctx* c, int fmt, int n, const uint32_t* tot, fg_batch_out* out) {
     out->n = n;
-    out->entry_name = c->h_entry_name;
-    out->entry_val = c->h_entry_val;
-    out->entry_meta = c->h_entry_meta;
+    for (const TableUse& u : kFormatTables[fmt]) {
+        const uint32_t rows = u.counter >= 0 ? tot[u.counter] : 0;
+        switch (u.table) {
+            case T_ENTRIES:
+                out->entry_name = host<fg_span>(c, T_ENTRIES, 0);
+                out->entry_val = host<uint64_t>(c, T_ENTRIES, 1);
+                out->entry_meta = host<uint8_t>(c, T_ENTRIES, 2);
+                out->n_entries = (int32_t)rows;
+                break;
+            case T_E8:
+                out->entries8 = host<uint64_t>(c, T_E8);
+                out->n_entries8 = (int32_t)rows;
+                break;
+            case T_ARENA:
+                out->arena = host<uint8_t>(c, T_ARENA);
+                out->arena_bytes = (int64_t)rows;
+                break;
+            case T_WIDE:
+                out->wide_rows = host<fg_wide_row>(c, T_WIDE);
+                out->n_wide = (int32_t)rows;
+                break;
+        }
+    }
     if (fmt == FG_FMT_RFC5424) {
-        out->n_entries = (int32_t)tot[fg::K5_WIDE_ENTRIES];
-        out->rows5424 = c->h_rows5;
-        out->entries8 = c->h_e8;
-        out->n_entries8 = (int32_t)tot[fg::K5_ENTRIES];
-        out->n_wide = (int32_t)tot[fg::K5_WIDE_ROWS];
-        out->wide_rows = c->h_wide;
-        out->arena = c->h_arena;
-        out->arena_bytes = (int64_t)tot[fg::K5_ARENA];
+        out->rows5424 = c->rows5.h;
         return;
     }
-    uint8_t* r = c->h_rows;
-    out->n_entries = (int32_t)tot[fg::K5_ENTRIES];
-    if (fmt == FG_FMT_RFC3164) {
-        out->n_entries = 0;
-        out->arena = c->h_arena;
-        out->arena_bytes = (int64_t)tot[fg::K5_ARENA];
-    }
+    uint8_t* r = c->rows.h;
     out->ts = (const double*)(r + col_off(c, C_TS));
     out->meta = (const uint32_t*)(r + col_off(c, C_META));
     out->hostname = (const fg_span*)(r + col_off(c, C_HOST));
@@ -531,14 +644,14 @@ void fill_out(fg_ctx* c, int fmt, int n, const uint32_t* tot, fg_batch_out* out)
 int copy_rows_d2h(fg_ctx* c, int fmt, int line0, int n, cudaStream_t s) {
     if (n <= 0) return FG_OK;
     if (fmt == FG_FMT_RFC5424) {
-        FG_CUDA(c, cudaMemcpyAsync(c->h_rows5 + line0, c->d_rows5 + 2 * (size_t)line0, (size_t)n * 32, cudaMemcpyDeviceToHost, s));
+        FG_CUDA(c, cudaMemcpyAsync(c->rows5.h + line0, c->rows5.d + line0, (size_t)n * 32, cudaMemcpyDeviceToHost, s));
         return FG_OK;
     }
     // ts and meta: one copy each; the 8-byte span columns share one pitch (8 * max_lines), so every run of consecutive
     // used span columns goes back as ONE 2-D copy (few large D2H operations disturb the concurrent H2D stream less)
     for (int col = C_TS; col <= C_META; ++col) {
         const size_t o = col_off(c, col) + (size_t)line0 * kColW[col];
-        FG_CUDA(c, cudaMemcpyAsync(c->h_rows + o, c->d_rows + o, (size_t)n * kColW[col], cudaMemcpyDeviceToHost, s));
+        FG_CUDA(c, cudaMemcpyAsync(c->rows.h + o, c->rows.d + o, (size_t)n * kColW[col], cudaMemcpyDeviceToHost, s));
     }
     const size_t pitch = (size_t)c->max_lines * 8;
     int col = C_HOST;
@@ -547,41 +660,11 @@ int copy_rows_d2h(fg_ctx* c, int fmt, int line0, int n, cudaStream_t s) {
         int end = col;
         while (end + 1 < C_COUNT && col_used(end + 1)) ++end;
         const size_t o = col_off(c, col) + (size_t)line0 * 8;
-        FG_CUDA(c, cudaMemcpy2DAsync(c->h_rows + o, pitch, c->d_rows + o, pitch, (size_t)n * 8, (size_t)(end - col + 1),
+        FG_CUDA(c, cudaMemcpy2DAsync(c->rows.h + o, pitch, c->rows.d + o, pitch, (size_t)n * 8, (size_t)(end - col + 1),
                                      cudaMemcpyDeviceToHost, s));
         col = end + 1;
     }
     return FG_OK;
-}
-
-int copy_entries_range(fg_ctx* c, size_t from, size_t to, cudaStream_t s) {
-    if (to <= from) return FG_OK;
-    const size_t k = to - from;
-    FG_CUDA(c, cudaMemcpyAsync(c->h_entry_name + from, c->d_entry_name + from, k * sizeof(int2), cudaMemcpyDeviceToHost, s));
-    FG_CUDA(c, cudaMemcpyAsync(c->h_entry_val + from, c->d_entry_val + from, k * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
-    FG_CUDA(c, cudaMemcpyAsync(c->h_entry_meta + from, c->d_entry_meta + from, k, cudaMemcpyDeviceToHost, s));
-    return FG_OK;
-}
-
-// side tables: the rows a chunk produced are the contiguous range [prev, cur) of each bump allocator
-int copy_tables_d2h(fg_ctx* c, int fmt, const uint32_t* prev, const uint32_t* cur, cudaStream_t s) {
-    if (fmt == FG_FMT_RFC3164) {
-        if (cur[fg::K5_ARENA] > prev[fg::K5_ARENA])
-            FG_CUDA(c, cudaMemcpyAsync(c->h_arena + prev[fg::K5_ARENA], c->d_arena + prev[fg::K5_ARENA],
-                                       (size_t)(cur[fg::K5_ARENA] - prev[fg::K5_ARENA]), cudaMemcpyDeviceToHost, s));
-        return FG_OK;
-    }
-    if (fmt != FG_FMT_RFC5424) return copy_entries_range(c, prev[fg::K5_ENTRIES], cur[fg::K5_ENTRIES], s);
-    if (cur[fg::K5_ENTRIES] > prev[fg::K5_ENTRIES])
-        FG_CUDA(c, cudaMemcpyAsync(c->h_e8 + prev[fg::K5_ENTRIES], c->d_e8 + prev[fg::K5_ENTRIES],
-                                   (size_t)(cur[fg::K5_ENTRIES] - prev[fg::K5_ENTRIES]) * 8, cudaMemcpyDeviceToHost, s));
-    if (cur[fg::K5_ARENA] > prev[fg::K5_ARENA])
-        FG_CUDA(c, cudaMemcpyAsync(c->h_arena + prev[fg::K5_ARENA], c->d_arena + prev[fg::K5_ARENA],
-                                   (size_t)(cur[fg::K5_ARENA] - prev[fg::K5_ARENA]), cudaMemcpyDeviceToHost, s));
-    if (cur[fg::K5_WIDE_ROWS] > prev[fg::K5_WIDE_ROWS])
-        FG_CUDA(c, cudaMemcpyAsync(c->h_wide + prev[fg::K5_WIDE_ROWS], c->d_wide + prev[fg::K5_WIDE_ROWS],
-                                   (size_t)(cur[fg::K5_WIDE_ROWS] - prev[fg::K5_WIDE_ROWS]) * sizeof(fg_wide_row), cudaMemcpyDeviceToHost, s));
-    return copy_entries_range(c, prev[fg::K5_WIDE_ENTRIES], cur[fg::K5_WIDE_ENTRIES], s);
 }
 
 bool is_pinned(const void* p) {
@@ -605,8 +688,8 @@ int h2d(fg_ctx* c, void* dst, const void* src, size_t bytes, bool pinned, int& b
         const size_t k = std::min(kBounceBytes, bytes - done);
         const int b = bounce_ix & 1;
         FG_CUDA(c, cudaEventSynchronize(c->bounce_ev[b]));
-        memcpy(c->h_bounce[b], (const uint8_t*)src + done, k);
-        FG_CUDA(c, cudaMemcpyAsync((uint8_t*)dst + done, c->h_bounce[b], k, cudaMemcpyHostToDevice, c->s_h2d));
+        memcpy(c->bounce[b].h, (const uint8_t*)src + done, k);
+        FG_CUDA(c, cudaMemcpyAsync((uint8_t*)dst + done, c->bounce[b].h, k, cudaMemcpyHostToDevice, c->s_h2d));
         FG_CUDA(c, cudaEventRecord(c->bounce_ev[b], c->s_h2d));
         done += k;
         ++bounce_ix;
@@ -614,23 +697,17 @@ int h2d(fg_ctx* c, void* dst, const void* src, size_t bytes, bool pinned, int& b
     return FG_OK;
 }
 
-int ensure_events(fg_ctx* c, int chunks) {
-    while ((int)c->ev_h2d.size() < chunks) {
-        cudaEvent_t a, b, d, e;
-        FG_CUDA(c, cudaEventCreateWithFlags(&a, cudaEventDisableTiming));
-        FG_CUDA(c, cudaEventCreate(&b));
-        FG_CUDA(c, cudaEventCreate(&d));
-        FG_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        c->ev_h2d.push_back(a);
-        c->ev_k0.push_back(b);
-        c->ev_k1.push_back(d);
-        c->ev_cnt.push_back(e);
+// events and counter snapshots for `steps` parse steps
+int ensure_steps(fg_ctx* c, int steps) {
+    while ((int)c->steps.size() < steps) {
+        StepEvents e;
+        FG_CUDA(c, create(e.h2d, cudaEventDisableTiming));
+        FG_CUDA(c, create(e.k0, cudaEventDefault));
+        FG_CUDA(c, create(e.k1, cudaEventDefault));
+        FG_CUDA(c, create(e.cnt, cudaEventDisableTiming));
+        c->steps.push_back(std::move(e));
     }
-    if (c->h_counts_cap < chunks) {
-        hfree(c->h_counts);
-        FG_CUDA(c, cudaHostAlloc(&c->h_counts, sizeof(uint32_t) * kCnt * (size_t)chunks, cudaHostAllocDefault));
-        c->h_counts_cap = chunks;
-    }
+    if (c->counts.n < (size_t)steps * fg::K5_COUNT) FG_CUDA(c, c->counts.alloc((size_t)steps * fg::K5_COUNT, HOST));
     return FG_OK;
 }
 
@@ -644,6 +721,117 @@ int check_batch(fg_ctx* c, const uint8_t* bytes, const int32_t* offsets, int32_t
         if (offsets[0] < 0 || offsets[n] < offsets[0]) return fail(c, FG_E_ARG, "offsets must be non-negative and non-decreasing");
         if ((size_t)offsets[n] > c->max_bytes) return fail(c, FG_E_CAPACITY, "batch has more bytes than max_batch_bytes");
     }
+    return FG_OK;
+}
+
+// A caller's batch of lines, uploaded chunk by chunk
+struct HostBatch {
+    const uint8_t* bytes;
+    const int32_t* offsets;
+    bool pin_b, pin_o;
+    int bounce_ix;
+};
+
+// Parse step k's input: H2D of lines [l0, l1) on s_h2d, then the device check of their offsets on s_comp
+int upload_chunk(fg_ctx* c, HostBatch& B, int k, int l0, int l1) {
+    const size_t b0 = (size_t)B.offsets[l0], b1 = (size_t)B.offsets[l1];
+    if (b1 < b0 || b1 > c->max_bytes) {
+        cudaDeviceSynchronize();
+        return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
+    }
+    if (int rc = h2d(c, c->bytes.d + b0, B.bytes + b0, b1 - b0, B.pin_b, B.bounce_ix)) return rc;
+    if (int rc = h2d(c, c->offsets.d + l0, B.offsets + l0, sizeof(int32_t) * (size_t)(l1 - l0 + 1), B.pin_o, B.bounce_ix)) return rc;
+    FG_CUDA(c, cudaEventRecord(c->steps[k].h2d, c->s_h2d));
+    FG_CUDA(c, cudaStreamWaitEvent(c->s_comp, c->steps[k].h2d, 0));
+    FG_CUDA(c, fg::launch_check_offsets(c->offsets.d + l0, l1 - l0, (long long)c->max_bytes, c->k.d + fg::K5_BAD_OFFSETS, c->s_comp));
+    return FG_OK;
+}
+
+// Parse step k of a pipelined call on stream s: the kernels over lines [l0, l0 + n) between the step's timing events
+// (with `encode`, the GELF encoder after the parse), the counter snapshot, then on s_d2h once the snapshot is in: the
+// rows, or the encoder's statuses and record offsets
+int parse_step(fg_ctx* c, int fmt, int k, int l0, int n, int tile, const uint8_t* invalid, int strip, cudaStream_t s,
+               bool encode) {
+    StepEvents& e = c->steps[k];
+    FG_CUDA(c, cudaEventRecord(e.k0, s));
+    if (int rc = launch_lines(c, fmt, l0, n, tile, invalid, strip, s)) return rc;
+    if (encode)
+        if (int rc = launch_encode(c, k, l0, n, tile, s)) return rc;
+    FG_CUDA(c, cudaEventRecord(e.k1, s));
+    FG_CUDA(c, cudaMemcpyAsync(c->counts.h + (size_t)k * fg::K5_COUNT, c->k.d, kCountBytes, cudaMemcpyDeviceToHost, s));
+    if (encode)
+        FG_CUDA(c, cudaMemcpyAsync(c->enc_base.h + k + 1, c->enc_base.d + k + 1, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    FG_CUDA(c, cudaEventRecord(e.cnt, s));
+    FG_CUDA(c, cudaStreamWaitEvent(c->s_d2h, e.cnt, 0));
+    if (!encode) return copy_rows_d2h(c, fmt, l0, n, c->s_d2h);
+    FG_CUDA(c, cudaMemcpyAsync(c->enc_status.h + l0, c->enc_status.d + l0, (size_t)n, cudaMemcpyDeviceToHost, c->s_d2h));
+    FG_CUDA(c, cudaMemcpyAsync(c->enc_offsets.h + l0, c->enc_offsets.d + l0, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, c->s_d2h));
+    return FG_OK;
+}
+
+// Waits for the counter snapshots of `steps` parse steps in order and copies what each step produced back on s_d2h
+// while later steps are still in flight: its range [prev, cur) of every side table, or with `encode` its encoded
+// records, the range [base(k), base(k+1)) of the output.  After an overflow nothing more is copied, but every snapshot
+// is still waited for.  total: the counters of the whole batch (the last snapshot).
+int drain(fg_ctx* c, int fmt, int steps, bool encode, uint32_t* total, bool& overflow) {
+    static const uint32_t zero[fg::K5_COUNT] = {};
+    const uint32_t* prev = zero;
+    overflow = false;
+    if (encode) c->enc_base.h[0] = 0;
+    for (int k = 0; k < steps; ++k) {
+        FG_CUDA(c, cudaEventSynchronize(c->steps[k].cnt));
+        const uint32_t* cur = c->counts.h + (size_t)k * fg::K5_COUNT;
+        const unsigned long long lo = encode ? c->enc_base.h[k] : 0, hi = encode ? c->enc_base.h[k + 1] : 0;
+        overflow = overflow || tables_overflow(c, fmt, cur) || hi > c->enc_out_cap;
+        if (overflow) continue;  // keep draining the events; the batch is redone
+        if (!encode) {
+            if (int rc = copy_tables_d2h(c, fmt, prev, cur, c->s_d2h)) return rc;
+        } else if (hi > lo) {
+            FG_CUDA(c, cudaMemcpyAsync(c->enc_out.h + lo, c->enc_out.d + lo, (size_t)(hi - lo), cudaMemcpyDeviceToHost, c->s_d2h));
+        }
+        prev = cur;
+    }
+    memcpy(total, steps ? c->counts.h + (size_t)(steps - 1) * fg::K5_COUNT : zero, kCountBytes);
+    return FG_OK;
+}
+
+// End of an attempt of a pipelined call: waits for s_d2h, rejects a batch whose offsets failed the device check, and
+// times the steps' kernels and the call so far
+int finish(fg_ctx* c, int steps, const uint32_t* total, std::chrono::steady_clock::time_point t_begin, float& kernel_ms,
+           float& total_ms) {
+    FG_CUDA(c, cudaStreamSynchronize(c->s_d2h));
+    if (total[fg::K5_BAD_OFFSETS]) return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
+    kernel_ms = 0.f;
+    for (int k = 0; k < steps; ++k) {
+        float ms = 0.f;
+        FG_CUDA(c, cudaEventElapsedTime(&ms, c->steps[k].k0, c->steps[k].k1));
+        kernel_ms += ms;
+    }
+    total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+    return FG_OK;
+}
+
+// One pass over the resident batch on s_comp.  Only the counters below the bad-offsets word are zeroed: a failed
+// fg_upload leaves that word set, which keeps the parse kernels inert.  `start`, when given, is recorded after the zeroing.
+int resident_pass(fg_ctx* c, int fmt, int tile, cudaEvent_t start, bool time_dominant) {
+    FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, sizeof(uint32_t) * fg::K5_BAD_OFFSETS, c->s_comp));
+    if (start) FG_CUDA(c, cudaEventRecord(start, c->s_comp));
+    return launch_lines(c, fmt, 0, c->res_n, tile, nullptr, 0, c->s_comp, time_dominant);
+}
+
+// After the resident passes since ev_a: ev_b, the counter block, and unless a table overflowed, the time from ev_a to
+// ev_b and the batch that fg_download returns
+int resident_end(fg_ctx* c, int fmt, uint32_t* total, float* ms, bool& overflow) {
+    FG_CUDA(c, cudaEventRecord(c->ev_b, c->s_comp));
+    FG_CUDA(c, cudaMemcpyAsync(total, c->k.d, kCountBytes, cudaMemcpyDeviceToHost, c->s_comp));
+    FG_CUDA(c, cudaStreamSynchronize(c->s_comp));
+    overflow = tables_overflow(c, fmt, total);
+    if (overflow) return FG_OK;
+    float t = 0.f;
+    FG_CUDA(c, cudaEventElapsedTime(&t, c->ev_a, c->ev_b));
+    if (ms) *ms = t;
+    c->res_fmt = fmt;
+    memcpy(c->res_tot, total, kCountBytes);
     return FG_OK;
 }
 
@@ -707,57 +895,70 @@ int build_static_items(fg_ctx* c) {
         lit_off.push_back((int32_t)blob.size());
         kind.push_back(it.kind);
     }
-    const size_t n = items.size();
-    const size_t o_key = (blob.size() + 15) & ~(size_t)15, o_lit = o_key + (n + 1) * 4, o_kind = o_lit + (n + 1) * 4;
-    std::vector<uint8_t> buf(o_kind + n * 4 + 16, 0);
-    memcpy(buf.data(), blob.data(), blob.size());
-    memcpy(buf.data() + o_key, key_off.data(), (n + 1) * 4);
-    memcpy(buf.data() + o_lit, lit_off.data(), (n + 1) * 4);
-    memcpy(buf.data() + o_kind, kind.data(), n * 4);
-    dfree(c->d_static_blob);
-    FG_CUDA(c, cudaMalloc(&c->d_static_blob, buf.size()));
-    FG_CUDA(c, cudaMemcpy(c->d_static_blob, buf.data(), buf.size(), cudaMemcpyHostToDevice));
-    c->n_static = (int)n;
-    c->d_static_key_off = (const int32_t*)(c->d_static_blob + o_key);
-    c->d_static_lit_off = (const int32_t*)(c->d_static_blob + o_lit);
-    c->d_static_kind = (const int32_t*)(c->d_static_blob + o_kind);
+    Packer p;
+    p.add(blob);  // at offset 0: the key and literal offsets index the blob itself
+    const size_t o_key = p.add(key_off), o_lit = p.add(lit_off), o_kind = p.add(kind);
+    if (int rc = p.upload(c, c->static_blob)) return rc;
+    const uint8_t* b = c->static_blob.d;
+    c->n_static = (int)items.size();
+    c->d_static_key_off = (const int32_t*)(b + o_key);
+    c->d_static_lit_off = (const int32_t*)(b + o_lit);
+    c->d_static_kind = (const int32_t*)(b + o_kind);
     return FG_OK;
 }
 
-int alloc_enc_out(fg_ctx* c, size_t cap) {
-    dfree(c->d_enc_out);
-    hfree(c->h_enc_out);
+int grow_enc_out(fg_ctx* c, size_t cap) {
     c->enc_out_cap = 0;
     cap = (cap + 4095) & ~(size_t)4095;
-    FG_CUDA(c, cudaMalloc(&c->d_enc_out, cap + 16));
-    FG_CUDA(c, cudaHostAlloc(&c->h_enc_out, cap + 16, cudaHostAllocDefault));
+    FG_CUDA(c, c->enc_out.alloc(cap + 16, BOTH));
     c->enc_out_cap = cap;
     return FG_OK;
 }
 
 int ensure_encoder(fg_ctx* c, int chunks) {
-    if (!c->d_enc_lens) {
-        FG_CUDA(c, cudaMalloc(&c->d_enc_lens, (size_t)c->max_lines * 4));
-        FG_CUDA(c, cudaMalloc(&c->d_enc_rel, (size_t)c->max_lines * 4));
-        FG_CUDA(c, cudaMalloc(&c->d_enc_offsets, ((size_t)c->max_lines + 1) * 8));
-        FG_CUDA(c, cudaHostAlloc(&c->h_enc_offsets, ((size_t)c->max_lines + 1) * 8, cudaHostAllocDefault));
-        FG_CUDA(c, cudaMalloc(&c->d_enc_status, (size_t)c->max_lines));
-        FG_CUDA(c, cudaHostAlloc(&c->h_enc_status, (size_t)c->max_lines, cudaHostAllocDefault));
+    const size_t L = (size_t)c->max_lines;
+    if (!c->enc_lens.d) {
+        FG_CUDA(c, c->enc_lens.alloc(L, DEV));
+        FG_CUDA(c, c->enc_rel.alloc(L, DEV));
+        FG_CUDA(c, c->enc_offsets.alloc(L + 1, BOTH));
+        FG_CUDA(c, c->enc_status.alloc(L, BOTH));
         c->scan_temp_bytes = fg::gelf_scan_temp_bytes(c->max_lines);
-        FG_CUDA(c, cudaMalloc(&c->d_scan_temp, c->scan_temp_bytes + 256));
+        FG_CUDA(c, c->scan_temp.alloc(c->scan_temp_bytes + 256, DEV));
     }
     if (!c->enc_out_cap)
-        if (int rc = alloc_enc_out(c, c->max_bytes * 2 + (size_t)c->max_lines * 200)) return rc;
-    if (c->enc_base_cap < chunks + 1) {
-        dfree(c->d_enc_base);
-        hfree(c->h_enc_base);
-        FG_CUDA(c, cudaMalloc(&c->d_enc_base, sizeof(unsigned long long) * ((size_t)chunks + 1)));
-        FG_CUDA(c, cudaHostAlloc(&c->h_enc_base, sizeof(unsigned long long) * ((size_t)chunks + 1), cudaHostAllocDefault));
-        c->enc_base_cap = chunks + 1;
-    }
-    if (!c->d_static_blob)
+        if (int rc = grow_enc_out(c, c->max_bytes * 2 + L * 200)) return rc;
+    if (c->enc_base.n < (size_t)chunks + 1) FG_CUDA(c, c->enc_base.alloc((size_t)chunks + 1, BOTH));
+    if (!c->static_blob.d)
         if (int rc = build_static_items(c)) return rc;
     return FG_OK;
+}
+
+// everything fg_create sets up on the device
+int init_device(fg_ctx* c, const fg_config* cfg) {
+    FG_CUDA(c, cudaSetDevice(c->device));
+    cudaDeviceProp prop;
+    FG_CUDA(c, cudaGetDeviceProperties(&prop, c->device));
+    const int max_tile = (int)std::min<size_t>(prop.sharedMemPerBlockOptin - 1024, 200 * 1024) & ~1023;
+    c->num_sms = prop.multiProcessorCount;
+    c->max_tile5 = (int)(((size_t)max_tile - 1024) * 8 / 9) & ~1023;  // tile + tile/8 bitmap + static shared memory
+    FG_CUDA(c, fg::configure_kernels(c->max_tile5));
+    FG_CUDA(c, create(c->s_h2d));
+    FG_CUDA(c, create(c->s_comp));
+    FG_CUDA(c, create(c->s_d2h));
+    FG_CUDA(c, create(c->ev_a, cudaEventDefault));
+    FG_CUDA(c, create(c->ev_b, cudaEventDefault));
+    FG_CUDA(c, create(c->ev_dom0, cudaEventDefault));
+    FG_CUDA(c, create(c->ev_dom1, cudaEventDefault));
+    FG_CUDA(c, c->bytes.alloc(c->max_bytes + kPad, DEV));
+    FG_CUDA(c, cudaMemset(c->bytes.d + c->max_bytes, 0, kPad));
+    FG_CUDA(c, c->offsets.alloc((size_t)c->max_lines + 1, DEV));
+    FG_CUDA(c, c->k.alloc(64, DEV));
+    FG_CUDA(c, cudaMemset(c->k.d, 0, 256));
+    for (int b = 0; b < 2; ++b) {
+        FG_CUDA(c, c->bounce[b].alloc(kBounceBytes, HOST));
+        FG_CUDA(c, create(c->bounce_ev[b], cudaEventDisableTiming));
+    }
+    return upload_ltsv_config(c, cfg);
 }
 
 }  // namespace
@@ -786,80 +987,11 @@ int fg_create(const fg_config* cfg, fg_ctx** out) {
     c->chunk_lines = (c->chunk_lines + 127) / 128 * 128;  // a multiple of every kernel's lines per CTA
     c->r3164_year = cfg->rfc3164_year;
     if (cfg->tzdir) c->tzdir = cfg->tzdir;
-#define FG_CREATE_CUDA(call)                                  \
-    do {                                                      \
-        cudaError_t _e = (call);                              \
-        if (_e != cudaSuccess) {                              \
-            fprintf(stderr, "flowgger_cuda: %s failed: %s\n", #call, cudaGetErrorString(_e)); \
-            fg_destroy(c);                                    \
-            return FG_E_CUDA;                                 \
-        }                                                     \
-    } while (0)
-    FG_CREATE_CUDA(cudaSetDevice(c->device));
-    cudaDeviceProp prop;
-    FG_CREATE_CUDA(cudaGetDeviceProperties(&prop, c->device));
-    c->max_tile = (int)std::min<size_t>(prop.sharedMemPerBlockOptin - 1024, 200 * 1024);
-    c->max_tile &= ~1023;
-    c->num_sms = prop.multiProcessorCount;
-    c->max_tile5 = (int)(((size_t)c->max_tile - 1024) * 8 / 9) & ~1023;  // tile + tile/8 bitmap + static shared memory
-    FG_CREATE_CUDA(fg::configure_kernels(c->max_tile, c->max_tile5));
-    FG_CREATE_CUDA(cudaStreamCreateWithFlags(&c->s_h2d, cudaStreamNonBlocking));
-    FG_CREATE_CUDA(cudaStreamCreateWithFlags(&c->s_comp, cudaStreamNonBlocking));
-    FG_CREATE_CUDA(cudaStreamCreateWithFlags(&c->s_d2h, cudaStreamNonBlocking));
-    FG_CREATE_CUDA(cudaEventCreate(&c->ev_a));
-    FG_CREATE_CUDA(cudaEventCreate(&c->ev_b));
-    FG_CREATE_CUDA(cudaEventCreate(&c->ev_dom0));
-    FG_CREATE_CUDA(cudaEventCreate(&c->ev_dom1));
-    FG_CREATE_CUDA(cudaMalloc(&c->d_bytes, c->max_bytes + kPad));
-    FG_CREATE_CUDA(cudaMemset(c->d_bytes + c->max_bytes, 0, kPad));
-    FG_CREATE_CUDA(cudaMalloc(&c->d_offsets, sizeof(int32_t) * ((size_t)c->max_lines + 1)));
-    FG_CREATE_CUDA(cudaMalloc(&c->d_k, 256));
-    FG_CREATE_CUDA(cudaMemset(c->d_k, 0, 256));
-    for (int b = 0; b < 2; ++b) {
-        FG_CREATE_CUDA(cudaHostAlloc(&c->h_bounce[b], kBounceBytes, cudaHostAllocDefault));
-        FG_CREATE_CUDA(cudaEventCreateWithFlags(&c->bounce_ev[b], cudaEventDisableTiming));
+    if (int rc = init_device(c, cfg)) {
+        fprintf(stderr, "flowgger_cuda: %s\n", c->last_error.c_str());
+        fg_destroy(c);
+        return rc;
     }
-    // LTSV schema / suffixes -> one device blob
-    {
-        std::vector<uint8_t> names, suffix;
-        std::vector<int32_t> name_off{0}, types;
-        const int ns = (cfg->ltsv_schema_names && cfg->ltsv_schema_types) ? cfg->ltsv_schema_len : 0;
-        for (int k = 0; k < ns; ++k) {
-            const char* s = cfg->ltsv_schema_names[k];
-            names.insert(names.end(), (const uint8_t*)s, (const uint8_t*)s + strlen(s));
-            name_off.push_back((int32_t)names.size());
-            types.push_back(cfg->ltsv_schema_types[k]);
-        }
-        fg::LtsvDeviceConfig& L = c->ltsv;
-        L.has_schema = (cfg->ltsv_has_schema || ns > 0) ? 1 : 0;
-        L.n_schema = ns;
-        L.suffix_present = 0;
-        L.suffix_off[0] = 0;
-        for (int t = 0; t < 5; ++t) {
-            const char* s = cfg->ltsv_suffix[t];
-            if (t > 0 && s) {
-                L.suffix_present |= 1u << t;
-                suffix.insert(suffix.end(), (const uint8_t*)s, (const uint8_t*)s + strlen(s));
-            }
-            L.suffix_off[t + 1] = (int32_t)suffix.size();
-        }
-        const size_t o_names = 0, o_off = (names.size() + 15) & ~(size_t)15;
-        const size_t o_types = o_off + ((name_off.size() * 4 + 15) & ~(size_t)15);
-        const size_t o_suf = o_types + ((types.size() * 4 + 15) & ~(size_t)15);
-        const size_t total = o_suf + suffix.size() + 16;
-        std::vector<uint8_t> blob(total, 0);
-        if (!names.empty()) memcpy(blob.data() + o_names, names.data(), names.size());
-        memcpy(blob.data() + o_off, name_off.data(), name_off.size() * 4);
-        if (!types.empty()) memcpy(blob.data() + o_types, types.data(), types.size() * 4);
-        if (!suffix.empty()) memcpy(blob.data() + o_suf, suffix.data(), suffix.size());
-        FG_CREATE_CUDA(cudaMalloc(&c->d_ltsv_blob, total));
-        FG_CREATE_CUDA(cudaMemcpy(c->d_ltsv_blob, blob.data(), total, cudaMemcpyHostToDevice));
-        L.names = c->d_ltsv_blob + o_names;
-        L.name_off = (const int32_t*)(c->d_ltsv_blob + o_off);
-        L.types = (const int32_t*)(c->d_ltsv_blob + o_types);
-        L.suffix = c->d_ltsv_blob + o_suf;
-    }
-#undef FG_CREATE_CUDA
     *out = c;
     return FG_OK;
 }
@@ -868,40 +1000,6 @@ void fg_destroy(fg_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
-    dfree(c->d_entry_name); dfree(c->d_entry_val); dfree(c->d_entry_meta);
-    hfree(c->h_entry_name); hfree(c->h_entry_val); hfree(c->h_entry_meta);
-    dfree(c->d_bytes); dfree(c->d_offsets); dfree(c->d_rows); dfree(c->d_k); dfree(c->d_flush);
-    dfree(c->d_rows5); hfree(c->h_rows5); dfree(c->d_e8); hfree(c->h_e8); dfree(c->d_esc_list); dfree(c->d_wide_list);
-    dfree(c->d_arena); hfree(c->h_arena); dfree(c->d_wide); hfree(c->h_wide);
-    dfree(c->d_enc_lens); dfree(c->d_enc_rel); dfree(c->d_enc_base); hfree(c->h_enc_base); dfree(c->d_enc_out); hfree(c->h_enc_out);
-    dfree(c->d_enc_offsets); hfree(c->h_enc_offsets); dfree(c->d_enc_status); hfree(c->h_enc_status); dfree(c->d_scan_temp);
-    dfree(c->d_static_blob);
-    dfree(c->d_seg); dfree(c->d_n_lines); dfree(c->d_invalid);
-    hfree(c->h_offsets); hfree(c->h_n_lines);
-    if (c->s_parse) cudaStreamDestroy(c->s_parse);
-    for (auto e : c->ev_split) cudaEventDestroy(e);
-    dfree(c->d_cum); hfree(c->h_cum);
-    if (c->ev_s0) cudaEventDestroy(c->ev_s0);
-    if (c->ev_s1) cudaEventDestroy(c->ev_s1);
-    dfree(c->d_tmp_name); dfree(c->d_tmp_val); dfree(c->d_tmp_meta);
-    dfree(c->d_ltsv_blob);
-    dfree(c->d_tz_blob);
-    hfree(c->h_rows); hfree(c->h_counts);
-    for (int b = 0; b < 2; ++b) {
-        hfree(c->h_bounce[b]);
-        if (c->bounce_ev[b]) cudaEventDestroy(c->bounce_ev[b]);
-    }
-    for (auto e : c->ev_h2d) cudaEventDestroy(e);
-    for (auto e : c->ev_k0) cudaEventDestroy(e);
-    for (auto e : c->ev_k1) cudaEventDestroy(e);
-    for (auto e : c->ev_cnt) cudaEventDestroy(e);
-    if (c->ev_a) cudaEventDestroy(c->ev_a);
-    if (c->ev_b) cudaEventDestroy(c->ev_b);
-    if (c->ev_dom0) cudaEventDestroy(c->ev_dom0);
-    if (c->ev_dom1) cudaEventDestroy(c->ev_dom1);
-    if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
-    if (c->s_comp) cudaStreamDestroy(c->s_comp);
-    if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
     delete c;
 }
 
@@ -921,80 +1019,39 @@ int fg_decode_batch(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_
                     fg_batch_out* out) {
     if (!c || !out) return FG_E_ARG;
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
-    if ((int)fmt < 0 || (int)fmt > 3) return fail(c, FG_E_ARG, "unknown format");
-    FG_CUDA(c, cudaSetDevice(c->device));
-    if (int rc = ensure_format(c, (int)fmt)) return rc;
-    c->call_year = current_year(c);
+    if (int rc = begin_call(c, fmt)) return rc;
     memset(out, 0, sizeof *out);
-    const uint32_t zero[kCnt] = {};
+    uint32_t total[fg::K5_COUNT] = {};
     if (n == 0) {
-        fill_out(c, fmt, 0, zero, out);
+        fill_out(c, fmt, 0, total, out);
         return FG_OK;
     }
     const auto t_begin = std::chrono::steady_clock::now();
-    const bool pin_b = is_pinned(bytes), pin_o = is_pinned(offsets);
+    HostBatch B{bytes, offsets, is_pinned(bytes), is_pinned(offsets), 0};
     const int C = c->chunk_lines;
     const int chunks = (n + C - 1) / C;
-    if (int rc = ensure_events(c, chunks)) return rc;
+    if (int rc = ensure_steps(c, chunks)) return rc;
     const int tile = pick_tile(c, (size_t)(offsets[n] - offsets[0]), n, (int)fmt);
     for (int attempt = 0; attempt < 2; ++attempt) {
-        FG_CUDA(c, cudaMemsetAsync(c->d_k, 0, sizeof(uint32_t) * kCnt, c->s_comp));
-        int bounce_ix = 0;
+        FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, kCountBytes, c->s_comp));
+        B.bounce_ix = 0;
         for (int k = 0; k < chunks; ++k) {
             const int l0 = k * C, l1 = std::min(n, l0 + C);
-            const size_t b0 = (size_t)offsets[l0], b1 = (size_t)offsets[l1];
-            if (b1 < b0 || b1 > c->max_bytes) {
-                cudaDeviceSynchronize();
-                return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
-            }
-            if (int rc = h2d(c, c->d_bytes + b0, bytes + b0, b1 - b0, pin_b, bounce_ix)) return rc;
-            if (int rc = h2d(c, c->d_offsets + l0, offsets + l0, sizeof(int32_t) * (size_t)(l1 - l0 + 1), pin_o, bounce_ix))
-                return rc;
-            FG_CUDA(c, cudaEventRecord(c->ev_h2d[k], c->s_h2d));
-            FG_CUDA(c, cudaStreamWaitEvent(c->s_comp, c->ev_h2d[k], 0));
-            FG_CUDA(c, fg::launch_check_offsets(c->d_offsets + l0, l1 - l0, (long long)c->max_bytes, c->d_k + kBadFlag, c->s_comp));
-            FG_CUDA(c, cudaEventRecord(c->ev_k0[k], c->s_comp));
-            if (int rc = launch_lines(c, (int)fmt, l0, l1 - l0, tile, nullptr, 0, c->s_comp)) return rc;
-            FG_CUDA(c, cudaEventRecord(c->ev_k1[k], c->s_comp));
-            FG_CUDA(c, cudaMemcpyAsync(c->h_counts + (size_t)k * kCnt, c->d_k, sizeof(uint32_t) * kCnt, cudaMemcpyDeviceToHost, c->s_comp));
-            FG_CUDA(c, cudaEventRecord(c->ev_cnt[k], c->s_comp));
-            FG_CUDA(c, cudaStreamWaitEvent(c->s_d2h, c->ev_cnt[k], 0));
-            if (int rc = copy_rows_d2h(c, fmt, l0, l1 - l0, c->s_d2h)) return rc;
+            if (int rc = upload_chunk(c, B, k, l0, l1)) return rc;
+            if (int rc = parse_step(c, fmt, k, l0, l1 - l0, tile, nullptr, 0, c->s_comp, false)) return rc;
         }
-        // side tables: chunk k's rows are the contiguous range [count(k-1), count(k)) of each bump allocator; a range is
-        // copied back as soon as its chunk has been parsed, while later chunks are still in flight
-        uint32_t prev[kCnt] = {};
-        bool overflow = false;
-        for (int k = 0; k < chunks; ++k) {
-            FG_CUDA(c, cudaEventSynchronize(c->ev_cnt[k]));
-            const uint32_t* cur = c->h_counts + (size_t)k * kCnt;
-            if (tables_overflow(c, (int)fmt, cur)) {
-                overflow = true;
-                continue;  // keep draining the events; the batch is redone below
-            }
-            if (!overflow) {
-                if (int rc = copy_tables_d2h(c, (int)fmt, prev, cur, c->s_d2h)) return rc;
-                memcpy(prev, cur, sizeof prev);
-            }
-        }
-        uint32_t total[kCnt];
-        memcpy(total, c->h_counts + (size_t)(chunks - 1) * kCnt, sizeof total);
-        FG_CUDA(c, cudaStreamSynchronize(c->s_d2h));
-        if (total[kBadFlag]) return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
+        bool overflow;
+        float kms, tms;
+        if (int rc = drain(c, fmt, chunks, false, total, overflow)) return rc;
+        if (int rc = finish(c, chunks, total, t_begin, kms, tms)) return rc;
         if (overflow) {
             // the allocators kept counting past the capacity: grow once to the exact need and redo
-            if (int rc = regrow_tables(c, (int)fmt, total)) return rc;
+            if (int rc = regrow_tables(c, fmt, total)) return rc;
             continue;
-        }
-        float kms = 0.f;
-        for (int k = 0; k < chunks; ++k) {
-            float ms = 0.f;
-            FG_CUDA(c, cudaEventElapsedTime(&ms, c->ev_k0[k], c->ev_k1[k]));
-            kms += ms;
         }
         fill_out(c, fmt, n, total, out);
         out->kernel_ms = kms;
-        out->total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+        out->total_ms = tms;
         return FG_OK;
     }
     return fail(c, FG_E_CAPACITY, "side table overflow after regrow");
@@ -1086,113 +1143,47 @@ int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const 
     if (!c || !out) return FG_E_ARG;
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
     if (fmt != FG_FMT_RFC5424) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
-    FG_CUDA(c, cudaSetDevice(c->device));
-    if (int rc = ensure_format(c, (int)fmt)) return rc;
-    c->call_year = current_year(c);
+    if (int rc = begin_call(c, fmt)) return rc;
     const int C = c->chunk_lines;
     const int chunks = n > 0 ? (n + C - 1) / C : 1;
     if (int rc = ensure_encoder(c, chunks)) return rc;
     memset(out, 0, sizeof *out);
-    out->bytes = c->h_enc_out;
-    out->offsets = c->h_enc_offsets;
-    out->status = c->h_enc_status;
+    out->bytes = c->enc_out.h;
+    out->offsets = c->enc_offsets.h;
+    out->status = c->enc_status.h;
     if (n == 0) {
-        c->h_enc_offsets[0] = 0;
+        c->enc_offsets.h[0] = 0;
         return FG_OK;
     }
     const auto t_begin = std::chrono::steady_clock::now();
-    const bool pin_b = is_pinned(bytes), pin_o = is_pinned(offsets);
-    if (int rc = ensure_events(c, chunks)) return rc;
+    HostBatch B{bytes, offsets, is_pinned(bytes), is_pinned(offsets), 0};
+    if (int rc = ensure_steps(c, chunks)) return rc;
     const int tile = pick_tile(c, (size_t)(offsets[n] - offsets[0]), n, (int)fmt);
     for (int attempt = 0; attempt < 3; ++attempt) {
-        FG_CUDA(c, cudaMemsetAsync(c->d_k, 0, sizeof(uint32_t) * kCnt, c->s_comp));
-        FG_CUDA(c, cudaMemsetAsync(c->d_enc_base, 0, sizeof(unsigned long long), c->s_comp));
-        int bounce_ix = 0;
+        FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, kCountBytes, c->s_comp));
+        FG_CUDA(c, cudaMemsetAsync(c->enc_base.d, 0, sizeof(unsigned long long), c->s_comp));
+        B.bounce_ix = 0;
         for (int k = 0; k < chunks; ++k) {
             const int l0 = k * C, l1 = std::min(n, l0 + C);
-            const size_t b0 = (size_t)offsets[l0], b1 = (size_t)offsets[l1];
-            if (b1 < b0 || b1 > c->max_bytes) {
-                cudaDeviceSynchronize();
-                return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
-            }
-            if (int rc = h2d(c, c->d_bytes + b0, bytes + b0, b1 - b0, pin_b, bounce_ix)) return rc;
-            if (int rc = h2d(c, c->d_offsets + l0, offsets + l0, sizeof(int32_t) * (size_t)(l1 - l0 + 1), pin_o, bounce_ix)) return rc;
-            FG_CUDA(c, cudaEventRecord(c->ev_h2d[k], c->s_h2d));
-            FG_CUDA(c, cudaStreamWaitEvent(c->s_comp, c->ev_h2d[k], 0));
-            FG_CUDA(c, fg::launch_check_offsets(c->d_offsets + l0, l1 - l0, (long long)c->max_bytes, c->d_k + kBadFlag, c->s_comp));
-            FG_CUDA(c, cudaEventRecord(c->ev_k0[k], c->s_comp));
-            if (int rc = launch_lines(c, (int)fmt, l0, l1 - l0, tile, nullptr, 0, c->s_comp)) return rc;
-            fg::GelfEncodeParams E;
-            E.bytes = c->d_bytes;
-            E.offsets = c->d_offsets + l0;
-            E.n = l1 - l0;
-            E.rows = c->d_rows5 + 2 * (size_t)l0;
-            E.entries = c->d_e8;
-            E.arena = c->d_arena;
-            E.wide_rows = c->d_wide;
-            E.wentry_name = c->d_entry_name;
-            E.wentry_val = c->d_entry_val;
-            E.wentry_meta = c->d_entry_meta;
-            E.static_blob = c->d_static_blob;
-            E.n_static = c->n_static;
-            E.static_key_off = c->d_static_key_off;
-            E.static_lit_off = c->d_static_lit_off;
-            E.static_kind = c->d_static_kind;
-            E.lens = c->d_enc_lens + l0;
-            E.rel = c->d_enc_rel + l0;
-            E.base = c->d_enc_base + k;
-            E.out = c->d_enc_out;
-            E.out_cap = c->enc_out_cap;
-            E.out_offsets = c->d_enc_offsets + l0;
-            E.status = c->d_enc_status + l0;
-            E.bad_offsets = c->d_k + kBadFlag;
-            E.entry_cap = (uint32_t)std::min<size_t>(c->e8_cap, 0xFFFFFFFFu);
-            E.wide_cap = (uint32_t)c->wide_cap;
-            E.wentry_cap = (uint32_t)std::min<size_t>(c->entry_cap, 0xFFFFFFFFu);
-            E.tile_bytes = std::min(4 * tile, c->max_tile5);  // the encoder's CTAs take 256 lines (4 x the parse kernel's 64)
-            FG_CUDA(c, fg::launch_gelf_encode(E, c->d_scan_temp, c->scan_temp_bytes, c->s_comp));
-            c->launches += 4;
-            FG_CUDA(c, cudaEventRecord(c->ev_k1[k], c->s_comp));
-            FG_CUDA(c, cudaMemcpyAsync(c->h_counts + (size_t)k * kCnt, c->d_k, sizeof(uint32_t) * kCnt, cudaMemcpyDeviceToHost, c->s_comp));
-            FG_CUDA(c, cudaMemcpyAsync(c->h_enc_base + k + 1, c->d_enc_base + k + 1, sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->s_comp));
-            FG_CUDA(c, cudaEventRecord(c->ev_cnt[k], c->s_comp));
-            FG_CUDA(c, cudaStreamWaitEvent(c->s_d2h, c->ev_cnt[k], 0));
-            FG_CUDA(c, cudaMemcpyAsync(c->h_enc_status + l0, c->d_enc_status + l0, (size_t)(l1 - l0), cudaMemcpyDeviceToHost, c->s_d2h));
-            FG_CUDA(c, cudaMemcpyAsync(c->h_enc_offsets + l0, c->d_enc_offsets + l0, (size_t)(l1 - l0 + 1) * 8, cudaMemcpyDeviceToHost, c->s_d2h));
+            if (int rc = upload_chunk(c, B, k, l0, l1)) return rc;
+            if (int rc = parse_step(c, fmt, k, l0, l1 - l0, tile, nullptr, 0, c->s_comp, true)) return rc;
         }
-        // encoded bytes: chunk k's records are the contiguous range [base(k), base(k+1)) of the output
-        c->h_enc_base[0] = 0;
-        bool overflow = false;
-        for (int k = 0; k < chunks; ++k) {
-            FG_CUDA(c, cudaEventSynchronize(c->ev_cnt[k]));
-            const uint32_t* cur = c->h_counts + (size_t)k * kCnt;
-            const unsigned long long lo = c->h_enc_base[k], hi = c->h_enc_base[k + 1];
-            if (tables_overflow(c, (int)fmt, cur) || hi > c->enc_out_cap) overflow = true;
-            if (!overflow && hi > lo)
-                FG_CUDA(c, cudaMemcpyAsync(c->h_enc_out + lo, c->d_enc_out + lo, (size_t)(hi - lo), cudaMemcpyDeviceToHost, c->s_d2h));
-        }
-        uint32_t total[kCnt];
-        memcpy(total, c->h_counts + (size_t)(chunks - 1) * kCnt, sizeof total);
-        FG_CUDA(c, cudaStreamSynchronize(c->s_d2h));
-        if (total[kBadFlag]) return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
+        uint32_t total[fg::K5_COUNT];
+        bool overflow;
+        float kms, tms;
+        if (int rc = drain(c, fmt, chunks, true, total, overflow)) return rc;
+        if (int rc = finish(c, chunks, total, t_begin, kms, tms)) return rc;
         if (overflow) {
-            if (tables_overflow(c, (int)fmt, total))
-                if (int rc = regrow_tables(c, (int)fmt, total)) return rc;
-            const unsigned long long need = c->h_enc_base[chunks];
+            if (int rc = regrow_tables(c, fmt, total)) return rc;
+            const unsigned long long need = c->enc_base.h[chunks];
             if (need > c->enc_out_cap)
-                if (int rc = alloc_enc_out(c, (size_t)need + (size_t)need / 8 + 4096)) return rc;
-            out->bytes = c->h_enc_out;
+                if (int rc = grow_enc_out(c, (size_t)need + (size_t)need / 8 + 4096)) return rc;
+            out->bytes = c->enc_out.h;
             continue;
-        }
-        float kms = 0.f;
-        for (int k = 0; k < chunks; ++k) {
-            float ms = 0.f;
-            FG_CUDA(c, cudaEventElapsedTime(&ms, c->ev_k0[k], c->ev_k1[k]));
-            kms += ms;
         }
         out->n = n;
         out->kernel_ms = kms;
-        out->total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+        out->total_ms = tms;
         return FG_OK;
     }
     return fail(c, FG_E_CAPACITY, "output / side table overflow after regrow");
@@ -1210,58 +1201,52 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
     const int strip = framing == FG_FRAME_NUL ? 2 : 1;
     if (nbytes < 0 || (nbytes > 0 && !stream)) return fail(c, FG_E_ARG, "null input");
     if ((size_t)nbytes > c->max_bytes) return fail(c, FG_E_CAPACITY, "stream has more bytes than max_batch_bytes");
-    FG_CUDA(c, cudaSetDevice(c->device));
-    if (int rc = ensure_format(c, (int)fmt)) return rc;
-    c->call_year = current_year(c);
+    if (int rc = begin_call(c, fmt)) return rc;
     const auto t_begin = std::chrono::steady_clock::now();
     constexpr long long kChunk = 64ll << 20;  // pipeline granularity in bytes (a multiple of the 8 KB framing segment)
     const int chunks = nbytes > 0 ? (int)((nbytes + kChunk - 1) / kChunk) : 1;
-    if (!c->d_seg) {
-        FG_CUDA(c, cudaMalloc(&c->d_seg, sizeof(uint32_t) * ((size_t)fg::split_segments((long long)c->max_bytes) + 16)));
-        FG_CUDA(c, cudaMalloc(&c->d_n_lines, 256));
-        FG_CUDA(c, cudaMalloc(&c->d_invalid, (size_t)c->max_lines + 64));
-        FG_CUDA(c, cudaHostAlloc(&c->h_offsets, sizeof(int32_t) * ((size_t)c->max_lines + 1), cudaHostAllocDefault));
-        FG_CUDA(c, cudaHostAlloc(&c->h_n_lines, 64, cudaHostAllocDefault));
-        FG_CUDA(c, cudaEventCreate(&c->ev_s0));
-        FG_CUDA(c, cudaEventCreate(&c->ev_s1));
-        FG_CUDA(c, cudaStreamCreateWithFlags(&c->s_parse, cudaStreamNonBlocking));
+    if (!c->seg.d) {
+        FG_CUDA(c, c->seg.alloc((size_t)fg::split_segments((long long)c->max_bytes) + 16, DEV));
+        FG_CUDA(c, c->n_lines.alloc(64, BOTH));
+        FG_CUDA(c, c->invalid.alloc((size_t)c->max_lines + 64, DEV));
+        FG_CUDA(c, c->split_offsets.alloc((size_t)c->max_lines + 1, HOST));
+        FG_CUDA(c, create(c->ev_s0, cudaEventDefault));
+        FG_CUDA(c, create(c->ev_s1, cudaEventDefault));
+        FG_CUDA(c, create(c->s_parse));
     }
     if ((int)c->ev_split.size() < chunks + 1) {
         const size_t want = (size_t)chunks + 1;
         while (c->ev_split.size() < want) {
-            cudaEvent_t e;
-            FG_CUDA(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            c->ev_split.push_back(e);
+            Event e;
+            FG_CUDA(c, create(e, cudaEventDisableTiming));
+            c->ev_split.push_back(std::move(e));
         }
-        dfree(c->d_cum);
-        hfree(c->h_cum);
-        FG_CUDA(c, cudaMalloc(&c->d_cum, sizeof(int32_t) * want));
-        FG_CUDA(c, cudaHostAlloc(&c->h_cum, sizeof(int32_t) * want, cudaHostAllocDefault));
+        FG_CUDA(c, c->cum.alloc(want, BOTH));
     }
-    if (int rc = ensure_events(c, chunks + 1)) return rc;
+    if (int rc = ensure_steps(c, chunks + 1)) return rc;
     memset(out, 0, sizeof *out);
     const bool pinned = nbytes > 0 && is_pinned(stream);
 
     for (int attempt = 0; attempt < 2; ++attempt) {
         // ---- enqueue, chunk by chunk: raw bytes -> HBM, then framing + UTF-8 validation of that chunk (no host dependency)
-        FG_CUDA(c, cudaMemsetAsync(c->d_n_lines + 8, 0, 4, c->s_comp));  // running newline count (uint32 at d_n_lines[8])
-        FG_CUDA(c, cudaMemsetAsync(c->d_invalid, 0, (size_t)c->max_lines, c->s_comp));
-        FG_CUDA(c, cudaMemsetAsync(c->d_k, 0, sizeof(uint32_t) * kCnt, c->s_comp));
+        FG_CUDA(c, cudaMemsetAsync(c->n_lines.d + 8, 0, 4, c->s_comp));  // running newline count (uint32 at n_lines[8])
+        FG_CUDA(c, cudaMemsetAsync(c->invalid.d, 0, (size_t)c->max_lines, c->s_comp));
+        FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, kCountBytes, c->s_comp));
         FG_CUDA(c, cudaEventRecord(c->ev_s0, c->s_comp));
         int bounce_ix = 0;
         for (int k = 0; k < chunks; ++k) {
             const long long c0 = (long long)k * kChunk, c1 = std::min<long long>(nbytes, c0 + kChunk);
             const bool last = k == chunks - 1;
-            if (int rc = h2d(c, c->d_bytes + c0, stream + c0, (size_t)(c1 - c0), pinned, bounce_ix)) return rc;
-            if (last) FG_CUDA(c, cudaMemsetAsync(c->d_bytes + nbytes, delim ? 0 : 0xFF, 64, c->s_h2d));  // whole-vector loads past the end see no delimiter
-            FG_CUDA(c, cudaEventRecord(c->ev_h2d[k], c->s_h2d));
-            FG_CUDA(c, cudaStreamWaitEvent(c->s_comp, c->ev_h2d[k], 0));
-            FG_CUDA(c, fg::launch_split_chunk(c->d_bytes, (long long)nbytes, c0, c1, last ? 1 : 0, c->d_seg, (uint32_t*)(c->d_n_lines + 8),
-                                              c->d_cum + k, c->d_offsets, c->d_n_lines, c->max_lines, c->d_invalid, delim, c->s_comp));
+            if (int rc = h2d(c, c->bytes.d + c0, stream + c0, (size_t)(c1 - c0), pinned, bounce_ix)) return rc;
+            if (last) FG_CUDA(c, cudaMemsetAsync(c->bytes.d + nbytes, delim ? 0 : 0xFF, 64, c->s_h2d));  // whole-vector loads past the end see no delimiter
+            FG_CUDA(c, cudaEventRecord(c->steps[k].h2d, c->s_h2d));
+            FG_CUDA(c, cudaStreamWaitEvent(c->s_comp, c->steps[k].h2d, 0));
+            FG_CUDA(c, fg::launch_split_chunk(c->bytes.d, (long long)nbytes, c0, c1, last ? 1 : 0, c->seg.d, (uint32_t*)(c->n_lines.d + 8),
+                                              c->cum.d + k, c->offsets.d, c->n_lines.d, c->max_lines, c->invalid.d, delim, c->s_comp));
             c->launches += 4;
-            FG_CUDA(c, cudaMemcpyAsync(c->h_cum + k, c->d_cum + k, 4, cudaMemcpyDeviceToHost, c->s_comp));
+            FG_CUDA(c, cudaMemcpyAsync(c->cum.h + k, c->cum.d + k, 4, cudaMemcpyDeviceToHost, c->s_comp));
             if (last) {
-                FG_CUDA(c, cudaMemcpyAsync(c->h_n_lines, c->d_n_lines, 4, cudaMemcpyDeviceToHost, c->s_comp));
+                FG_CUDA(c, cudaMemcpyAsync(c->n_lines.h, c->n_lines.d, 4, cudaMemcpyDeviceToHost, c->s_comp));
                 FG_CUDA(c, cudaEventRecord(c->ev_s1, c->s_comp));
             }
             FG_CUDA(c, cudaEventRecord(c->ev_split[k], c->s_comp));
@@ -1275,10 +1260,10 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
         for (int k = 0; k < chunks; ++k) {
             const int dep = std::min(k + 1, chunks - 1);
             FG_CUDA(c, cudaEventSynchronize(c->ev_split[dep]));
-            int32_t upto = c->h_cum[k];
+            int32_t upto = c->cum.h[k];
             if (upto < 0) { over = true; break; }
             if (k == chunks - 1) {
-                n = *c->h_n_lines;
+                n = *c->n_lines.h;
                 if (n < 0) { over = true; break; }
                 upto = n;  // includes an unterminated last line
             }
@@ -1287,13 +1272,7 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
                 const size_t span_bytes = (size_t)std::min<long long>(nbytes, (long long)(k + 1) * kChunk) - (size_t)((long long)k * kChunk);
                 const int tile = pick_tile(c, std::max<size_t>(span_bytes, 1), cnt, (int)fmt);
                 FG_CUDA(c, cudaStreamWaitEvent(c->s_parse, c->ev_split[dep], 0));
-                FG_CUDA(c, cudaEventRecord(c->ev_k0[nparse], c->s_parse));
-                if (int rc = launch_lines(c, (int)fmt, done_lines, cnt, tile, c->d_invalid + done_lines, strip, c->s_parse)) return rc;
-                FG_CUDA(c, cudaEventRecord(c->ev_k1[nparse], c->s_parse));
-                FG_CUDA(c, cudaMemcpyAsync(c->h_counts + (size_t)nparse * kCnt, c->d_k, sizeof(uint32_t) * kCnt, cudaMemcpyDeviceToHost, c->s_parse));
-                FG_CUDA(c, cudaEventRecord(c->ev_cnt[nparse], c->s_parse));
-                FG_CUDA(c, cudaStreamWaitEvent(c->s_d2h, c->ev_cnt[nparse], 0));
-                if (int rc = copy_rows_d2h(c, fmt, done_lines, cnt, c->s_d2h)) return rc;
+                if (int rc = parse_step(c, fmt, nparse, done_lines, cnt, tile, c->invalid.d + done_lines, strip, c->s_parse, false)) return rc;
                 ++nparse;
                 done_lines = upto;
             }
@@ -1303,37 +1282,22 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
             return fail(c, FG_E_CAPACITY, "stream has more lines than max_batch_lines");
         }
         // ---- side table ranges, line offsets
-        uint32_t prev[kCnt] = {}, total[kCnt] = {};
-        bool overflow = false;
-        for (int j = 0; j < nparse; ++j) {
-            FG_CUDA(c, cudaEventSynchronize(c->ev_cnt[j]));
-            const uint32_t* cur = c->h_counts + (size_t)j * kCnt;
-            memcpy(total, cur, sizeof total);
-            if (tables_overflow(c, (int)fmt, cur)) { overflow = true; continue; }
-            if (!overflow) {
-                if (int rc = copy_tables_d2h(c, (int)fmt, prev, cur, c->s_d2h)) return rc;
-                memcpy(prev, cur, sizeof prev);
-            }
-        }
+        uint32_t total[fg::K5_COUNT];
+        bool overflow;
+        float kms, tms;
+        if (int rc = drain(c, fmt, nparse, false, total, overflow)) return rc;
+        if (!overflow)
+            FG_CUDA(c, cudaMemcpyAsync(c->split_offsets.h, c->offsets.d, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->s_d2h));
+        if (int rc = finish(c, nparse, total, t_begin, kms, tms)) return rc;
         if (overflow) {
-            FG_CUDA(c, cudaDeviceSynchronize());
-            if (int rc = regrow_tables(c, (int)fmt, total)) return rc;
+            if (int rc = regrow_tables(c, fmt, total)) return rc;
             continue;
-        }
-        FG_CUDA(c, cudaStreamSynchronize(c->s_parse));
-        FG_CUDA(c, cudaMemcpyAsync(c->h_offsets, c->d_offsets, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->s_d2h));
-        FG_CUDA(c, cudaStreamSynchronize(c->s_d2h));
-        float kms = 0.f;
-        for (int j = 0; j < nparse; ++j) {
-            float ms = 0.f;
-            FG_CUDA(c, cudaEventElapsedTime(&ms, c->ev_k0[j], c->ev_k1[j]));
-            kms += ms;
         }
         FG_CUDA(c, cudaEventElapsedTime(&c->last_split_ms, c->ev_s0, c->ev_s1));  // includes waiting for the H2D chunks
         fill_out(c, fmt, n, total, out);
-        out->line_offsets = c->h_offsets;
+        out->line_offsets = c->split_offsets.h;
         out->kernel_ms = kms;
-        out->total_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+        out->total_ms = tms;
         return FG_OK;
     }
     return fail(c, FG_E_CAPACITY, "side table overflow after regrow");
@@ -1344,16 +1308,16 @@ int fg_upload(fg_ctx* c, const uint8_t* bytes, const int32_t* offsets, int32_t n
     FG_CUDA(c, cudaSetDevice(c->device));
     if (n > 0) {
         const size_t b0 = (size_t)offsets[0], b1 = (size_t)offsets[n];
-        FG_CUDA(c, cudaMemcpy(c->d_bytes + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice));
-        FG_CUDA(c, cudaMemcpy(c->d_offsets, offsets, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyHostToDevice));
+        FG_CUDA(c, cudaMemcpy(c->bytes.d + b0, bytes + b0, b1 - b0, cudaMemcpyHostToDevice));
+        FG_CUDA(c, cudaMemcpy(c->offsets.d, offsets, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyHostToDevice));
         c->res_bytes = b1 - b0;
     } else {
         c->res_bytes = 0;
     }
-    FG_CUDA(c, cudaMemset(c->d_k, 0, sizeof(uint32_t) * kCnt));
-    FG_CUDA(c, fg::launch_check_offsets(c->d_offsets, n, (long long)c->max_bytes, c->d_k + kBadFlag, c->s_comp));
+    FG_CUDA(c, cudaMemset(c->k.d, 0, kCountBytes));
+    FG_CUDA(c, fg::launch_check_offsets(c->offsets.d, n, (long long)c->max_bytes, c->k.d + fg::K5_BAD_OFFSETS, c->s_comp));
     uint32_t bad = 0;
-    FG_CUDA(c, cudaMemcpyAsync(&bad, c->d_k + kBadFlag, 4, cudaMemcpyDeviceToHost, c->s_comp));
+    FG_CUDA(c, cudaMemcpyAsync(&bad, c->k.d + fg::K5_BAD_OFFSETS, 4, cudaMemcpyDeviceToHost, c->s_comp));
     FG_CUDA(c, cudaStreamSynchronize(c->s_comp));
     if (bad) return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
     c->res_n = n;
@@ -1363,28 +1327,17 @@ int fg_upload(fg_ctx* c, const uint8_t* bytes, const int32_t* offsets, int32_t n
 
 int fg_parse_resident(fg_ctx* c, fg_format fmt, float* kernel_ms) {
     if (!c) return FG_E_ARG;
-    if ((int)fmt < 0 || (int)fmt > 3) return fail(c, FG_E_ARG, "unknown format");
-    FG_CUDA(c, cudaSetDevice(c->device));
-    if (int rc = ensure_format(c, (int)fmt)) return rc;
-    c->call_year = current_year(c);
+    if (int rc = begin_call(c, fmt)) return rc;
     for (int attempt = 0; attempt < 2; ++attempt) {
-        FG_CUDA(c, cudaMemsetAsync(c->d_k, 0, sizeof(uint32_t) * kBadFlag, c->s_comp));
-        FG_CUDA(c, cudaEventRecord(c->ev_a, c->s_comp));
-        if (int rc = launch_lines(c, (int)fmt, 0, c->res_n, pick_tile(c, c->res_bytes, c->res_n, (int)fmt), nullptr, 0, c->s_comp, true)) return rc;
-        FG_CUDA(c, cudaEventRecord(c->ev_b, c->s_comp));
-        uint32_t total[kCnt] = {};
-        FG_CUDA(c, cudaMemcpyAsync(total, c->d_k, sizeof total, cudaMemcpyDeviceToHost, c->s_comp));
-        FG_CUDA(c, cudaStreamSynchronize(c->s_comp));
-        if (tables_overflow(c, (int)fmt, total)) {
+        if (int rc = resident_pass(c, (int)fmt, pick_tile(c, c->res_bytes, c->res_n, (int)fmt), c->ev_a, true)) return rc;
+        uint32_t total[fg::K5_COUNT] = {};
+        bool overflow;
+        if (int rc = resident_end(c, (int)fmt, total, kernel_ms, overflow)) return rc;
+        if (overflow) {
             if (int rc = regrow_tables(c, (int)fmt, total)) return rc;
             continue;
         }
-        float ms = 0.f;
-        FG_CUDA(c, cudaEventElapsedTime(&ms, c->ev_a, c->ev_b));
-        if (kernel_ms) *kernel_ms = ms;
         FG_CUDA(c, cudaEventElapsedTime(&c->last_dom_ms, c->ev_dom0, c->ev_dom1));
-        c->res_fmt = (int)fmt;
-        memcpy(c->res_tot, total, sizeof total);
         return FG_OK;
     }
     return fail(c, FG_E_CAPACITY, "side table overflow after regrow");
@@ -1394,28 +1347,16 @@ int fg_parse_resident(fg_ctx* c, fg_format fmt, float* kernel_ms) {
 // total_ms = CUDA-event time from before the first launch to after the last one.
 int fg_parse_resident_n(fg_ctx* c, fg_format fmt, int32_t k, float* total_ms) {
     if (!c || k < 1) return FG_E_ARG;
-    if ((int)fmt < 0 || (int)fmt > 3) return fail(c, FG_E_ARG, "unknown format");
-    FG_CUDA(c, cudaSetDevice(c->device));
-    if (int rc = ensure_format(c, (int)fmt)) return rc;
-    c->call_year = current_year(c);
+    if (int rc = begin_call(c, fmt)) return rc;
     // the side tables must already be large enough (one fg_parse_resident warm-up regrows them): checked after the loop
     const int tile = pick_tile(c, c->res_bytes, c->res_n, (int)fmt);
     FG_CUDA(c, cudaEventRecord(c->ev_a, c->s_comp));
-    for (int32_t it = 0; it < k; ++it) {
-        FG_CUDA(c, cudaMemsetAsync(c->d_k, 0, sizeof(uint32_t) * kBadFlag, c->s_comp));
-        if (int rc = launch_lines(c, (int)fmt, 0, c->res_n, tile, nullptr, 0, c->s_comp)) return rc;
-    }
-    FG_CUDA(c, cudaEventRecord(c->ev_b, c->s_comp));
-    uint32_t total[kCnt] = {};
-    FG_CUDA(c, cudaMemcpyAsync(total, c->d_k, sizeof total, cudaMemcpyDeviceToHost, c->s_comp));
-    FG_CUDA(c, cudaStreamSynchronize(c->s_comp));
-    if (tables_overflow(c, (int)fmt, total))
-        return fail(c, FG_E_CAPACITY, "side table too small: call fg_parse_resident once before fg_parse_resident_n");
-    float ms = 0.f;
-    FG_CUDA(c, cudaEventElapsedTime(&ms, c->ev_a, c->ev_b));
-    if (total_ms) *total_ms = ms;
-    c->res_fmt = (int)fmt;
-    memcpy(c->res_tot, total, sizeof total);
+    for (int32_t it = 0; it < k; ++it)
+        if (int rc = resident_pass(c, (int)fmt, tile, nullptr, false)) return rc;
+    uint32_t total[fg::K5_COUNT] = {};
+    bool overflow;
+    if (int rc = resident_end(c, (int)fmt, total, total_ms, overflow)) return rc;
+    if (overflow) return fail(c, FG_E_CAPACITY, "side table too small: call fg_parse_resident once before fg_parse_resident_n");
     return FG_OK;
 }
 
@@ -1424,7 +1365,7 @@ int fg_download(fg_ctx* c, fg_format fmt, fg_batch_out* out) {
     if (c->res_fmt != (int)fmt) return fail(c, FG_E_ARG, "no resident parse of this format to download");
     FG_CUDA(c, cudaSetDevice(c->device));
     memset(out, 0, sizeof *out);
-    const uint32_t zero[kCnt] = {};
+    const uint32_t zero[fg::K5_COUNT] = {};
     if (int rc = copy_rows_d2h(c, fmt, 0, c->res_n, c->s_d2h)) return rc;
     if (int rc = copy_tables_d2h(c, (int)fmt, zero, c->res_tot, c->s_d2h)) return rc;
     FG_CUDA(c, cudaStreamSynchronize(c->s_d2h));
@@ -1435,8 +1376,8 @@ int fg_download(fg_ctx* c, fg_format fmt, fg_batch_out* out) {
 int fg_flush_l2(fg_ctx* c) {
     if (!c) return FG_E_ARG;
     FG_CUDA(c, cudaSetDevice(c->device));
-    if (!c->d_flush) FG_CUDA(c, cudaMalloc(&c->d_flush, kL2FlushBytes));
-    FG_CUDA(c, cudaMemsetAsync(c->d_flush, 0x5A, kL2FlushBytes, c->s_comp));
+    if (!c->flush.d) FG_CUDA(c, c->flush.alloc(kL2FlushBytes, DEV));
+    FG_CUDA(c, cudaMemsetAsync(c->flush.d, 0x5A, kL2FlushBytes, c->s_comp));
     FG_CUDA(c, cudaStreamSynchronize(c->s_comp));
     return FG_OK;
 }

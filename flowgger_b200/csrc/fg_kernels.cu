@@ -16,8 +16,7 @@
 
 namespace fg {
 
-cudaError_t configure_kernels(int max_tile_bytes, int max_tile5424) {
-    (void)max_tile_bytes;
+cudaError_t configure_kernels(int max_tile5424) {
     cudaError_t e = configure_parse5424(max_tile5424);
     if (e != cudaSuccess) return e;
     e = configure_gelf_encode(max_tile5424);

@@ -103,7 +103,9 @@ struct WideRow {
 };
 static_assert(sizeof(WideRow) == 72, "WideRow must be 72 bytes");
 
-enum { K5_ENTRIES = 0, K5_ARENA = 1, K5_WIDE_ROWS = 2, K5_WIDE_ENTRIES = 3, K5_ESC_LIST = 4, K5_WIDE_LIST = 5, K5_COUNT = 8 };
+// the counter block of a context: K5_BAD_OFFSETS is set by check_offsets_kernel; K5_COUNT words are snapshotted per chunk
+enum { K5_ENTRIES = 0, K5_ARENA = 1, K5_WIDE_ROWS = 2, K5_WIDE_ENTRIES = 3, K5_ESC_LIST = 4, K5_WIDE_LIST = 5, K5_BAD_OFFSETS = 6,
+       K5_COUNT = 8 };
 
 struct Parse5424Params {
     const uint8_t* bytes;
@@ -232,7 +234,7 @@ cudaError_t launch_parse3164(const ParseParams& p, cudaStream_t stream);
 cudaError_t configure_parse3164(int max_tile_bytes);
 // offsets[0 .. n] must be non-decreasing and within [0, max_bytes]; otherwise *flag |= 1 (the parse kernels then return at once)
 cudaError_t launch_check_offsets(const int32_t* d_offsets, int n, long long max_bytes, uint32_t* d_flag, cudaStream_t stream);
-cudaError_t configure_kernels(int max_tile_bytes, int max_tile5424);
+cudaError_t configure_kernels(int max_tile5424);
 const char* kernel_build_info();
 
 // device-side line framing + UTF-8 validation (fg_split.cu)
