@@ -88,6 +88,9 @@ def decode_dump(native, data: np.ndarray, offsets: np.ndarray, tile_bytes: int =
     try:
         buf, offs = dump_records(native.FMT_RFC5424, out, data, offsets)
         info = {"n_entries8": out.n_entries8, "n_wide": out.n_wide, "arena_bytes": out.arena_bytes, "n_entries": out.n_entries}
+        # the batch line of every wide row (WideRow.line, the first int32 of each 72-byte row)
+        rows = np.ctypeslib.as_array(C.cast(out.wide_rows, C.POINTER(C.c_int32)), shape=(out.n_wide * 18,)) if out.n_wide else []
+        info["wide_lines"] = {int(x) for x in rows[::18]}
     finally:
         lib().emu5424_free(C.byref(out))
     return buf, offs, info
@@ -117,13 +120,13 @@ def ltsv_decode_dump(native, data: np.ndarray, offsets: np.ndarray, schema: dict
     for k, v in (suffixes or {}).items():
         suf[LTSV_TYPES[k.lower()]] = v.encode()
     csuf = (C.c_char_p * 5)(*suf)
-    info = (C.c_int32 * 2)()
+    info = (C.c_int32 * 3)()
     lib().emu_ltsv_decode(C.c_void_p(data.ctypes.data), C.c_void_p(offsets.ctypes.data), n, tile_bytes, strip_eol,
                           C.c_void_p(invalid.ctypes.data) if invalid is not None else None, 1 if schema is not None else 0,
                           len(items), names, types, csuf, C.byref(out), info)
     try:
         buf, offs = dump_records(native.FMT_LTSV, out, data, offsets, ltsv_suffix=suf)
-        d = {"n_entries": out.n_entries, "rounds": int(info[0]), "direct": int(info[1])}
+        d = {"n_entries": out.n_entries, "rounds": int(info[0]), "direct": int(info[1]), "schema_staged": bool(info[2])}
     finally:
         lib().emu_ltsv_free(C.byref(out))
     return buf, offs, d

@@ -62,7 +62,7 @@ uint32_t emu_ltsv_classify16(const uint8_t* p) {
 // schema: n_schema names (NUL-terminated) + types; suffix[5] indexed by fg_ltsv_type (nullptr = none)
 int emu_ltsv_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int32_t tile_bytes, int32_t strip_eol,
                     const uint8_t* invalid, int32_t has_schema, int32_t n_schema, const char* const* names, const int32_t* types,
-                    const char* const* suffix, fg_batch_out* out, int32_t* info /* [2]: rounds, direct-path lines */) {
+                    const char* const* suffix, fg_batch_out* out, int32_t* info /* [3]: rounds, direct-path lines, schema staged */) {
     Tables* T = new Tables();
     const size_t nn = (size_t)std::max(n, 1);
     T->ts.resize(nn); T->meta.resize(nn); T->host.resize(nn); T->msg.resize(nn); T->full.resize(nn); T->sd.resize(nn);
@@ -93,7 +93,11 @@ int emu_ltsv_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
     const bool typed = cfg.has_schema != 0;
     uint32_t first[8], len_mask;
     fg::lt_schema_filters(cfg.names, cfg.name_off, cfg.n_schema, len_mask, first);
-    const fg::LtsvSchemaView S = {cfg.names, cfg.name_off, cfg.types, cfg.n_schema, len_mask, first};
+    // parse_ltsv_kernel stages a schema of <= 64 keys, <= 1024 name bytes and <= 64 suffix bytes in shared memory with the
+    // two filters; a larger one is read from global memory with the filters off
+    const bool staged = cfg.n_schema <= 64 && name_blob.size() <= 1024 && suffix_blob.size() <= 64;
+    const fg::LtsvSchemaView S = {cfg.names, cfg.name_off, cfg.types, cfg.n_schema, staged ? len_mask : 0xFFFFFFFFu,
+                                  staged ? first : nullptr};
 
     const int64_t total_bytes = n > 0 ? offsets[n] : 0;
     std::vector<uint8_t> tile((size_t)tile_bytes + 64);
@@ -298,7 +302,7 @@ int emu_ltsv_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
     out->entry_val = T->eval.data();
     out->entry_meta = T->emeta.data();
     out->line_offsets = (const int32_t*)T;  // owner handle for emu_ltsv_free
-    if (info) { info[0] = T->rounds; info[1] = T->direct; }
+    if (info) { info[0] = T->rounds; info[1] = T->direct; info[2] = typed && staged ? 1 : 0; }
     return 0;
 }
 
