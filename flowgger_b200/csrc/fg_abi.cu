@@ -769,30 +769,55 @@ int parse_step(fg_ctx* c, int fmt, int k, int l0, int n, int tile, const uint8_t
     return FG_OK;
 }
 
-// Waits for the counter snapshots of `steps` parse steps in order and copies what each step produced back on s_d2h
-// while later steps are still in flight: its range [prev, cur) of every side table, or with `encode` its encoded
-// records, the range [base(k), base(k+1)) of the output.  After an overflow nothing more is copied, but every snapshot
-// is still waited for.  total: the counters of the whole batch (the last snapshot).
-int drain(fg_ctx* c, int fmt, int steps, bool encode, uint32_t* total, bool& overflow) {
-    static const uint32_t zero[fg::K5_COUNT] = {};
-    const uint32_t* prev = zero;
-    overflow = false;
+const uint32_t kZeroCounts[fg::K5_COUNT] = {};
+
+// How far the drain of one attempt has got: the next parse step, the counters the last drained one left, whether a step
+// overflowed
+struct Drain {
+    bool encode;
+    int next = 0;
+    const uint32_t* prev = kZeroCounts;
+    bool overflow = false;
+};
+
+Drain begin_drain(fg_ctx* c, bool encode) {
     if (encode) c->enc_base.h[0] = 0;
-    for (int k = 0; k < steps; ++k) {
+    return Drain{encode};
+}
+
+// Waits for the counter snapshots of the parse steps before `upto` in order and copies what each step produced back on
+// s_d2h while later steps are still in flight: its range [prev, cur) of every side table, or with `encode` its encoded
+// records, the range [base(k), base(k+1)) of the output.  After an overflow nothing more is copied, but every snapshot
+// is still waited for.
+int drain_upto(fg_ctx* c, int fmt, int upto, Drain& d) {
+    for (; d.next < upto; ++d.next) {
+        const int k = d.next;
         FG_CUDA(c, cudaEventSynchronize(c->steps[k].cnt));
         const uint32_t* cur = c->counts.h + (size_t)k * fg::K5_COUNT;
-        const unsigned long long lo = encode ? c->enc_base.h[k] : 0, hi = encode ? c->enc_base.h[k + 1] : 0;
-        overflow = overflow || tables_overflow(c, fmt, cur) || hi > c->enc_out_cap;
-        if (overflow) continue;  // keep draining the events; the batch is redone
-        if (!encode) {
-            if (int rc = copy_tables_d2h(c, fmt, prev, cur, c->s_d2h)) return rc;
+        const unsigned long long lo = d.encode ? c->enc_base.h[k] : 0, hi = d.encode ? c->enc_base.h[k + 1] : 0;
+        d.overflow = d.overflow || tables_overflow(c, fmt, cur) || hi > c->enc_out_cap;
+        if (d.overflow) continue;  // keep draining the events; the batch is redone
+        if (!d.encode) {
+            if (int rc = copy_tables_d2h(c, fmt, d.prev, cur, c->s_d2h)) return rc;
         } else if (hi > lo) {
             FG_CUDA(c, cudaMemcpyAsync(c->enc_out.h + lo, c->enc_out.d + lo, (size_t)(hi - lo), cudaMemcpyDeviceToHost, c->s_d2h));
         }
-        prev = cur;
+        d.prev = cur;
     }
-    memcpy(total, steps ? c->counts.h + (size_t)(steps - 1) * fg::K5_COUNT : zero, kCountBytes);
     return FG_OK;
+}
+
+// drain_upto over the rest of `steps` parse steps.  total: the counters of the whole batch (the last snapshot).
+int end_drain(fg_ctx* c, int fmt, int steps, Drain& d, uint32_t* total, bool& overflow) {
+    if (int rc = drain_upto(c, fmt, steps, d)) return rc;
+    overflow = d.overflow;
+    memcpy(total, steps ? c->counts.h + (size_t)(steps - 1) * fg::K5_COUNT : kZeroCounts, kCountBytes);
+    return FG_OK;
+}
+
+int drain(fg_ctx* c, int fmt, int steps, bool encode, uint32_t* total, bool& overflow) {
+    Drain d = begin_drain(c, encode);
+    return end_drain(c, fmt, steps, d, total, overflow);
 }
 
 // End of an attempt of a pipelined call: waits for s_d2h, rejects a batch whose offsets failed the device check, and
@@ -1189,22 +1214,27 @@ int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const 
     return fail(c, FG_E_CAPACITY, "output / side table overflow after regrow");
 }
 
-int fg_split_decode(fg_ctx* c, fg_format fmt, const uint8_t* stream, int64_t nbytes, fg_batch_out* out) {
-    return fg_split_decode_framed(c, fmt, FG_FRAME_LINE, stream, nbytes, out);
-}
+}  // extern "C"
 
-int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_batch_out* out) {
-    if (!c || !out) return FG_E_ARG;
-    if ((int)fmt < 0 || (int)fmt > 3) return fail(c, FG_E_ARG, "unknown format");
+namespace {
+
+// Raw stream -> framing + UTF-8 check (split kernels on s_comp, 64 MiB chunk by chunk) -> parse kernels on s_parse,
+// and with `encode` the GELF encoder after each parse step.  Without `encode` the rows and side tables come back, with
+// it only the encoded records; the line offsets come back into split_offsets.h either way.  n: records framed; total,
+// kernel_ms, total_ms: as drain and finish give them.
+int split_stream(fg_ctx* c, int fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, bool encode, int32_t& n,
+                 uint32_t* total, float& kernel_ms, float& total_ms) {
     if (framing != FG_FRAME_LINE && framing != FG_FRAME_NUL) return fail(c, FG_E_ARG, "unknown framing");
     const int delim = framing == FG_FRAME_NUL ? 0 : '\n';
     const int strip = framing == FG_FRAME_NUL ? 2 : 1;
     if (nbytes < 0 || (nbytes > 0 && !stream)) return fail(c, FG_E_ARG, "null input");
     if ((size_t)nbytes > c->max_bytes) return fail(c, FG_E_CAPACITY, "stream has more bytes than max_batch_bytes");
-    if (int rc = begin_call(c, fmt)) return rc;
+    if (int rc = begin_call(c, (fg_format)fmt)) return rc;
     const auto t_begin = std::chrono::steady_clock::now();
     constexpr long long kChunk = 64ll << 20;  // pipeline granularity in bytes (a multiple of the 8 KB framing segment)
     const int chunks = nbytes > 0 ? (int)((nbytes + kChunk - 1) / kChunk) : 1;
+    if (encode)
+        if (int rc = ensure_encoder(c, chunks)) return rc;  // at most one parse step per chunk
     if (!c->seg.d) {
         FG_CUDA(c, c->seg.alloc((size_t)fg::split_segments((long long)c->max_bytes) + 16, DEV));
         FG_CUDA(c, c->n_lines.alloc(64, BOTH));
@@ -1224,14 +1254,15 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
         FG_CUDA(c, c->cum.alloc(want, BOTH));
     }
     if (int rc = ensure_steps(c, chunks + 1)) return rc;
-    memset(out, 0, sizeof *out);
     const bool pinned = nbytes > 0 && is_pinned(stream);
 
-    for (int attempt = 0; attempt < 2; ++attempt) {
+    const int attempts = encode ? 3 : 2;  // encode: a side table and the output buffer may each overflow once
+    for (int attempt = 0; attempt < attempts; ++attempt) {
         // ---- enqueue, chunk by chunk: raw bytes -> HBM, then framing + UTF-8 validation of that chunk (no host dependency)
         FG_CUDA(c, cudaMemsetAsync(c->n_lines.d + 8, 0, 4, c->s_comp));  // running newline count (uint32 at n_lines[8])
         FG_CUDA(c, cudaMemsetAsync(c->invalid.d, 0, (size_t)c->max_lines, c->s_comp));
         FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, kCountBytes, c->s_comp));
+        if (encode) FG_CUDA(c, cudaMemsetAsync(c->enc_base.d, 0, sizeof(unsigned long long), c->s_comp));
         FG_CUDA(c, cudaEventRecord(c->ev_s0, c->s_comp));
         int bounce_ix = 0;
         for (int k = 0; k < chunks; ++k) {
@@ -1252,11 +1283,13 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
             FG_CUDA(c, cudaEventRecord(c->ev_split[k], c->s_comp));
         }
         // ---- parse the lines that END in chunk k once chunk k+1 has been validated too (a sequence that starts in the
-        //      last 16 bytes of a chunk is checked with the next one); rows go back while later chunks are still in flight
+        //      last 16 bytes of a chunk is checked with the next one); what a step produced goes back while later chunks
+        //      are still in flight
         int32_t done_lines = 0;
-        int32_t n = 0;
+        n = 0;
         int nparse = 0;
         bool over = false;
+        Drain d = begin_drain(c, encode);
         for (int k = 0; k < chunks; ++k) {
             const int dep = std::min(k + 1, chunks - 1);
             FG_CUDA(c, cudaEventSynchronize(c->ev_split[dep]));
@@ -1272,35 +1305,77 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
                 const size_t span_bytes = (size_t)std::min<long long>(nbytes, (long long)(k + 1) * kChunk) - (size_t)((long long)k * kChunk);
                 const int tile = pick_tile(c, std::max<size_t>(span_bytes, 1), cnt, (int)fmt);
                 FG_CUDA(c, cudaStreamWaitEvent(c->s_parse, c->ev_split[dep], 0));
-                if (int rc = parse_step(c, fmt, nparse, done_lines, cnt, tile, c->invalid.d + done_lines, strip, c->s_parse, false)) return rc;
+                if (int rc = parse_step(c, fmt, nparse, done_lines, cnt, tile, c->invalid.d + done_lines, strip, c->s_parse, encode)) return rc;
                 ++nparse;
                 done_lines = upto;
+                if (int rc = drain_upto(c, fmt, nparse - 1, d)) return rc;  // the step before this one
             }
         }
         if (over) {
             FG_CUDA(c, cudaDeviceSynchronize());
             return fail(c, FG_E_CAPACITY, "stream has more lines than max_batch_lines");
         }
-        // ---- side table ranges, line offsets
-        uint32_t total[fg::K5_COUNT];
+        // ---- the last step, line offsets
         bool overflow;
-        float kms, tms;
-        if (int rc = drain(c, fmt, nparse, false, total, overflow)) return rc;
+        if (int rc = end_drain(c, fmt, nparse, d, total, overflow)) return rc;
         if (!overflow)
             FG_CUDA(c, cudaMemcpyAsync(c->split_offsets.h, c->offsets.d, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->s_d2h));
-        if (int rc = finish(c, nparse, total, t_begin, kms, tms)) return rc;
+        if (int rc = finish(c, nparse, total, t_begin, kernel_ms, total_ms)) return rc;
         if (overflow) {
             if (int rc = regrow_tables(c, fmt, total)) return rc;
+            const unsigned long long need = encode ? c->enc_base.h[nparse] : 0;
+            if (need > c->enc_out_cap)
+                if (int rc = grow_enc_out(c, (size_t)need + (size_t)need / 8 + 4096)) return rc;
             continue;
         }
         FG_CUDA(c, cudaEventElapsedTime(&c->last_split_ms, c->ev_s0, c->ev_s1));  // includes waiting for the H2D chunks
-        fill_out(c, fmt, n, total, out);
-        out->line_offsets = c->split_offsets.h;
-        out->kernel_ms = kms;
-        out->total_ms = tms;
+        if (encode && nparse == 0) c->enc_offsets.h[0] = 0;
         return FG_OK;
     }
-    return fail(c, FG_E_CAPACITY, "side table overflow after regrow");
+    return fail(c, FG_E_CAPACITY, encode ? "output / side table overflow after regrow" : "side table overflow after regrow");
+}
+
+}  // namespace
+
+extern "C" {
+
+int fg_split_decode(fg_ctx* c, fg_format fmt, const uint8_t* stream, int64_t nbytes, fg_batch_out* out) {
+    return fg_split_decode_framed(c, fmt, FG_FRAME_LINE, stream, nbytes, out);
+}
+
+int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_batch_out* out) {
+    if (!c || !out) return FG_E_ARG;
+    if ((int)fmt < 0 || (int)fmt > 3) return fail(c, FG_E_ARG, "unknown format");
+    int32_t n;
+    uint32_t total[fg::K5_COUNT];
+    float kms, tms;
+    if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, false, n, total, kms, tms)) return rc;
+    memset(out, 0, sizeof *out);
+    fill_out(c, fmt, n, total, out);
+    out->line_offsets = c->split_offsets.h;
+    out->kernel_ms = kms;
+    out->total_ms = tms;
+    return FG_OK;
+}
+
+// framing + decode (RFC5424) + GelfEncoder::encode on the device: only the encoded records and the line offsets come back
+int fg_split_decode_encode_gelf(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
+                                const int32_t** line_offsets) {
+    if (!c || !out || !line_offsets) return FG_E_ARG;
+    if (fmt != FG_FMT_RFC5424) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
+    int32_t n;
+    uint32_t total[fg::K5_COUNT];
+    float kms, tms;
+    if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, true, n, total, kms, tms)) return rc;
+    memset(out, 0, sizeof *out);
+    out->n = n;
+    out->bytes = c->enc_out.h;
+    out->offsets = c->enc_offsets.h;
+    out->status = c->enc_status.h;
+    out->kernel_ms = kms;
+    out->total_ms = tms;
+    *line_offsets = c->split_offsets.h;
+    return FG_OK;
 }
 
 int fg_upload(fg_ctx* c, const uint8_t* bytes, const int32_t* offsets, int32_t n) {

@@ -224,21 +224,34 @@ void CudaBatchDecoder::decode_batch(const uint8_t* bytes, const int32_t* offsets
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_batch: ") + fg_last_error(ctx_));
 }
 
+void CudaBatchDecoder::set_gelf_extra(const std::vector<std::pair<std::string, std::string>>& extra) {
+    if (extra_valid_ && extra == extra_set_) return;
+    std::vector<const char*> k, v;
+    for (const auto& kv : extra) {
+        k.push_back(kv.first.c_str());
+        v.push_back(kv.second.c_str());
+    }
+    if (fg_set_gelf_extra(ctx_, (int32_t)extra.size(), k.data(), v.data()) != FG_OK)
+        throw std::runtime_error(std::string("fg_set_gelf_extra: ") + fg_last_error(ctx_));
+    extra_set_ = extra;
+    extra_valid_ = true;
+}
+
 void CudaBatchDecoder::decode_encode_gelf(const uint8_t* bytes, const int32_t* offsets, int32_t n,
                                           const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out) {
-    if (!extra_valid_ || extra != extra_set_) {
-        std::vector<const char*> k, v;
-        for (const auto& kv : extra) {
-            k.push_back(kv.first.c_str());
-            v.push_back(kv.second.c_str());
-        }
-        if (fg_set_gelf_extra(ctx_, (int32_t)extra.size(), k.data(), v.data()) != FG_OK)
-            throw std::runtime_error(std::string("fg_set_gelf_extra: ") + fg_last_error(ctx_));
-        extra_set_ = extra;
-        extra_valid_ = true;
-    }
+    set_gelf_extra(extra);
     const int rc = fg_decode_encode_gelf(ctx_, fmt_, bytes, offsets, n, out);
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_encode_gelf: ") + fg_last_error(ctx_));
+}
+
+bool CudaBatchDecoder::try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
+                                                    const std::vector<std::pair<std::string, std::string>>& extra,
+                                                    fg_encoded_out* out, const int32_t** line_offsets) {
+    set_gelf_extra(extra);
+    const int rc = fg_split_decode_encode_gelf(ctx_, fmt_, framing, stream, nbytes, out, line_offsets);
+    if (rc == FG_E_CAPACITY) return false;
+    if (rc != FG_OK) throw std::runtime_error(std::string("fg_split_decode_encode_gelf: ") + fg_last_error(ctx_));
+    return true;
 }
 
 static std::string_view span_sv(const uint8_t* bytes, fg_span s) {
@@ -255,10 +268,18 @@ void CudaBatchDecoder::split_decode(const uint8_t* stream, int64_t nbytes, fg_ba
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_split_decode: ") + fg_last_error(ctx_));
 }
 
-// extent of line i of a split-mode result without its "\n" / "\r\n" terminator (BufRead::lines)
-static void split_extent(const fg_batch_out& out, const uint8_t* stream, int32_t i, int32_t& lo, int32_t& hi, fg_framing framing) {
-    lo = out.line_offsets[i];
-    hi = out.line_offsets[i + 1];
+bool CudaBatchDecoder::try_split_decode(const uint8_t* stream, int64_t nbytes, fg_batch_out* out, fg_framing framing) {
+    const int rc = fg_split_decode_framed(ctx_, fmt_, framing, stream, nbytes, out);
+    if (rc == FG_E_CAPACITY) return false;
+    if (rc != FG_OK) throw std::runtime_error(std::string("fg_split_decode: ") + fg_last_error(ctx_));
+    return true;
+}
+
+// extent of record i of a split-mode result without its terminator: "\n" / "\r\n" (BufRead::lines) or NUL
+// (BufRead::split(0)); line_offsets as fg_batch_out.line_offsets
+static void split_extent(const int32_t* line_offsets, const uint8_t* stream, int32_t i, int32_t& lo, int32_t& hi, fg_framing framing) {
+    lo = line_offsets[i];
+    hi = line_offsets[i + 1];
     if (framing == FG_FRAME_NUL) {  // BufRead::split(0): only the NUL goes
         if (hi > lo && stream[hi - 1] == 0) --hi;
         return;
@@ -476,11 +497,21 @@ RecordBatcher::RecordBatcher(const Decoder& decoder, const Encoder& encoder, std
     arena_.reserve((size_t)max_bytes_);
 }
 
-void RecordBatcher::report(const char* e, std::string_view line) {
+// "{err}: [{line.trim()}]" for a rejected record; `quiet_blank`: nothing for a blank one (the NUL splitter)
+static void report_error(std::ostream& err, const char* e, std::string_view line, bool quiet_blank) {
     const std::string_view t = rust_trim(line);
-    if (quiet_blank_ && t.empty()) return;  // nul_splitter.rs:41-45
-    err_ << e << ": [" << t << "]\n";       // line_splitter.rs:37-39, nul_splitter.rs:43, syslen_splitter.rs:37
+    if (quiet_blank && t.empty()) return;  // nul_splitter.rs:41-45
+    err << e << ": [" << t << "]\n";       // line_splitter.rs:37-39, nul_splitter.rs:43, syslen_splitter.rs:37
 }
+
+// GELF without "timestamp": the reference stamps the record with the wall clock (gelf_decoder.rs:109 -> utils/mod.rs:16-21)
+static double wall_clock_ts() {
+    timespec tsn;
+    clock_gettime(CLOCK_REALTIME, &tsn);
+    return (double)tsn.tv_sec + (double)tsn.tv_nsec / 1e9;
+}
+
+void RecordBatcher::report(const char* e, std::string_view line) { report_error(err_, e, line, quiet_blank_); }
 
 void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
     const int32_t n = (int32_t)offsets_.size() - 1;
@@ -515,11 +546,7 @@ void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
             for (const auto& s : fx) out_ << s << "\n";
             const char* e = r.err;
             if (!e) {
-                if (FG_META_FLAGS(row_meta(out, i)) & FG_FLAG_TS_MISSING) {
-                    timespec tsn;
-                    clock_gettime(CLOCK_REALTIME, &tsn);
-                    r.record.ts = (double)tsn.tv_sec + (double)tsn.tv_nsec / 1e9;
-                }
+                if (FG_META_FLAGS(row_meta(out, i)) & FG_FLAG_TS_MISSING) r.record.ts = wall_clock_ts();
                 std::vector<uint8_t> enc;
                 if (encoder_.encode(std::move(r.record), enc, &e)) {
                     tx_(std::move(enc));
@@ -553,30 +580,152 @@ void RecordBatcher::push(std::string_view line) {
     invalid_before_.push_back(0);
 }
 
+namespace {
+
+constexpr const char* kInvalidUtf8 = "Invalid UTF-8 input";  // line_splitter.rs:23, nul_splitter.rs:25
+
+bool is_invalid_utf8_status(fg_format fmt, uint32_t status) {
+    const char* s = status ? fg_error_string(fmt, status) : nullptr;
+    return s && strcmp(s, kInvalidUtf8) == 0;
+}
+
+// The line and NUL splitters: raw blocks of the stream, each cut after its last delimiter, are framed, checked for UTF-8
+// and decoded on the device (fg_split_decode_framed), with a CudaGelfEncoder on an RFC5424 decoder also encoded there
+// (fg_split_decode_encode_gelf).  Records, stderr and stdout come out in stream order, exactly as the reference's
+// splitter + decoder + encoder give them.
+class BlockSplitter {
+   public:
+    BlockSplitter(fg_framing framing, bool quiet_blank, const Decoder& decoder, const Encoder& encoder,
+                  const std::function<void(std::vector<uint8_t>&&)>& tx, std::ostream& err_out, std::ostream& std_out)
+        : framing_(framing), delim_(framing == FG_FRAME_NUL ? 0 : '\n'), quiet_blank_(quiet_blank), gpu_(decoder.batch()),
+          encoder_(encoder), fused_(dynamic_cast<const CudaGelfEncoder*>(&encoder)), tx_(tx), err_(err_out), out_(std_out) {}
+
+    // blocks of up to `block_bytes` (at most the context's max_batch_bytes); a record longer than that grows its block
+    void run(std::istream& in, int64_t block_bytes) {
+        block_bytes = std::max<int64_t>(1, std::min(block_bytes, gpu_->capacity_bytes()));
+        std::vector<uint8_t> buf((size_t)block_bytes);
+        size_t have = 0;  // bytes in buf: the tail of the last block, then what was read since
+        for (bool eof = false; !eof;) {
+            if (have == buf.size()) buf.resize(buf.size() * 2);  // no delimiter in a whole buffer: a record longer than a block
+            const size_t want = buf.size() - have;
+            in.read((char*)buf.data() + have, (std::streamsize)want);
+            const size_t got = (size_t)in.gcount();
+            have += got;
+            eof = got < want;
+            size_t cut = have;  // at the end of the stream an unterminated last record is still a record
+            if (!eof) {
+                const auto last = std::find(buf.rbegin() + (std::ptrdiff_t)(buf.size() - have), buf.rend(), delim_);
+                if (last == buf.rend()) continue;
+                cut = (size_t)(buf.rend() - last);
+            }
+            if (cut) decode(gpu_.get(), buf.data(), (int64_t)cut);
+            memmove(buf.data(), buf.data() + cut, have - cut);
+            have -= cut;
+            if (buf.size() > (size_t)block_bytes && have < (size_t)block_bytes) buf.resize((size_t)block_bytes);
+        }
+    }
+
+   private:
+    // records [p, p + n) in order: on `gpu` when they fit, else in two halves cut at a delimiter near the middle; a lone
+    // record longer than the context gets a context of its own, sized for it (rare, slow, correct), as RecordBatcher::push
+    void decode(CudaBatchDecoder* gpu, const uint8_t* p, int64_t n) {
+        if (n <= gpu->capacity_bytes() && decode_on(gpu, p, n)) return;
+        if (const int64_t cut = cut_near_middle(p, n)) {
+            decode(gpu, p, cut);
+            decode(gpu, p + cut, n - cut);
+            return;
+        }
+        std::unique_ptr<CudaBatchDecoder> big = gpu->make_sized(n + 4096, 64);
+        if (!decode_on(big.get(), p, n)) throw std::runtime_error("a record does not fit a context sized for it");
+    }
+
+    // the end of a record near the middle of [p, p + n), 0 when the block is one record (its last byte ends the last record)
+    int64_t cut_near_middle(const uint8_t* p, int64_t n) const {
+        const uint8_t *mid = p + n / 2, *end = p + n - 1;
+        const uint8_t* f = std::find(mid, end, delim_);
+        if (f != end) return f - p + 1;
+        for (const uint8_t* b = mid; b > p;)
+            if (*--b == delim_) return b - p + 1;
+        return 0;
+    }
+
+    // false: more records than the context holds, nothing was emitted
+    bool decode_on(CudaBatchDecoder* gpu, const uint8_t* p, int64_t n) {
+        std::lock_guard<std::mutex> guard(gpu->mutex());  // held until every record of the block has been emitted
+        const fg_format fmt = gpu->format();
+        if (fused_ != nullptr && fmt == FG_FMT_RFC5424) {
+            // framing + decode + encode on the device (line_splitter.rs:17-52 fused): only the encoded records come back
+            fg_encoded_out eo;
+            const int32_t* lines;
+            if (!gpu->try_split_decode_encode_gelf(p, n, framing_, fused_->extra(), &eo, &lines)) return false;
+            for (int32_t i = 0; i < eo.n; ++i) {
+                if (eo.status[i] == 0) {
+                    tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
+                    continue;
+                }
+                int32_t lo, hi;
+                split_extent(lines, p, i, lo, hi, framing_);
+                reject(fmt, eo.status[i], fg_error_string(fmt, eo.status[i]), p, lo, hi);
+            }
+            return true;
+        }
+        fg_batch_out out;
+        if (!gpu->try_split_decode(p, n, &out, framing_)) return false;
+        std::vector<std::string> fx;
+        for (int32_t i = 0; i < out.n; ++i) {
+            int32_t lo, hi;
+            split_extent(out.line_offsets, p, i, lo, hi, framing_);
+            const uint32_t meta = row_meta(out, i);
+            if (is_invalid_utf8_status(fmt, FG_META_STATUS(meta))) {
+                err_ << kInvalidUtf8 << "\n";
+                continue;
+            }
+            fx.clear();
+            DecodeResult r = gpu->materialize_line(out, p, lo, hi, i, &fx);
+            for (const auto& s : fx) out_ << s << "\n";
+            const char* e = r.err;
+            if (!e) {
+                if (FG_META_FLAGS(meta) & FG_FLAG_TS_MISSING) r.record.ts = wall_clock_ts();
+                std::vector<uint8_t> enc;
+                if (encoder_.encode(std::move(r.record), enc, &e)) {
+                    tx_(std::move(enc));
+                    continue;
+                }
+            }
+            reject(fmt, FG_META_STATUS(meta), e, p, lo, hi);
+        }
+        return true;
+    }
+
+    // "Invalid UTF-8 input" (line_splitter.rs:22-25), else "{err}: [{trim}]"
+    void reject(fg_format fmt, uint32_t status, const char* e, const uint8_t* p, int32_t lo, int32_t hi) {
+        if (is_invalid_utf8_status(fmt, status)) err_ << kInvalidUtf8 << "\n";
+        else report_error(err_, e, std::string_view((const char*)p + lo, (size_t)(hi - lo)), quiet_blank_);
+    }
+
+    fg_framing framing_;
+    uint8_t delim_;
+    bool quiet_blank_;
+    std::shared_ptr<CudaBatchDecoder> gpu_;
+    const Encoder& encoder_;
+    const CudaGelfEncoder* fused_;
+    const std::function<void(std::vector<uint8_t>&&)>& tx_;
+    std::ostream& err_;
+    std::ostream& out_;
+};
+
+}  // namespace
+
 void BatchingLineSplitter::run(std::istream& in, const std::function<void(std::vector<uint8_t>&&)>& tx,
                                const Decoder& decoder, const Encoder& encoder, std::ostream& err_out,
                                std::ostream& std_out) const {
-    RecordBatcher batch(decoder, encoder, tx, err_out, std_out, RecordBatcher::Limits{lim_.max_lines, lim_.max_bytes});
-    std::string line;
-    while (std::getline(in, line)) {
-        // BufRead::lines: the '\n' is gone; a '\r' is stripped only when it preceded a '\n'
-        if (!in.eof() && !line.empty() && line.back() == '\r') line.pop_back();
-        if (!is_valid_utf8((const uint8_t*)line.data(), line.size())) batch.invalid_utf8();  // printed in stream order at the flush
-        else batch.push(line);
-    }
-    batch.flush();
+    BlockSplitter(FG_FRAME_LINE, false, decoder, encoder, tx, err_out, std_out).run(in, lim_.max_bytes);
 }
 
 // splitter/nul_splitter.rs:18-47: records end at a NUL byte; the message for a rejected record is suppressed when the record is blank
 void BatchingNulSplitter::run(std::istream& in, const std::function<void(std::vector<uint8_t>&&)>& tx, const Decoder& decoder,
                               const Encoder& encoder, std::ostream& err_out, std::ostream& std_out) const {
-    RecordBatcher batch(decoder, encoder, tx, err_out, std_out, RecordBatcher::Limits{lim_.max_lines, lim_.max_bytes}, true);
-    std::string rec;
-    while (std::getline(in, rec, '\0')) {
-        if (!is_valid_utf8((const uint8_t*)rec.data(), rec.size())) batch.invalid_utf8();
-        else batch.push(rec);
-    }
-    batch.flush();
+    BlockSplitter(FG_FRAME_NUL, true, decoder, encoder, tx, err_out, std_out).run(in, lim_.max_bytes);
 }
 
 // splitter/syslen_splitter.rs:17-57: octet-counted framing "<len> <record>"; the chain of lengths is sequential by nature, so
@@ -918,7 +1067,7 @@ int fgh_split_dump(void* d, int framing, const uint8_t* stream, int64_t nbytes, 
         std::vector<std::string> fx;
         for (int32_t i = 0; i < n; ++i) {
             int32_t lo, hi;
-            split_extent(out, stream, i, lo, hi, (fg_framing)framing);
+            split_extent(out.line_offsets, stream, i, lo, hi, (fg_framing)framing);
             fx.clear();
             DecodeResult r = dec->materialize_line(out, stream, lo, hi, i, &fx);
             const bool now = r.ok() && (FG_META_FLAGS(row_meta(out, i)) & FG_FLAG_TS_MISSING);
@@ -990,10 +1139,11 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
     }
 }
 
-// BatchingLineSplitter with output.format = "gelf" (fused decode + encode): text in, one JSON record per line out
+// BatchingLineSplitter (framing 0) or BatchingNulSplitter (framing 1) with output.format = "gelf" (fused decode + encode):
+// text in, one JSON record per line out
 int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
                           const char* const* keys, const char* const* vals, uint8_t** out_records, int64_t* out_records_len,
-                          uint8_t** out_stderr, int64_t* out_stderr_len) {
+                          uint8_t** out_stderr, int64_t* out_stderr_len, int framing) {
     struct Shared : Decoder {
         std::shared_ptr<CudaBatchDecoder> b;
         DecodeResult decode(std::string_view) const override { return {}; }
@@ -1007,13 +1157,14 @@ int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max
     BatchingLineSplitter::Limits lim;
     lim.max_lines = max_lines;
     lim.max_bytes = max_bytes;
-    BatchingLineSplitter sp(lim);
     std::string in((const char*)text, (size_t)len);
     std::istringstream is(in);
     std::ostringstream es, os;
     std::string records;
     try {
-        sp.run(is, [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); }, dec, enc, es, os);
+        auto tx = [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); };
+        if (framing == 1) BatchingNulSplitter(lim).run(is, tx, dec, enc, es, os);  // input.framing = "nul"
+        else BatchingLineSplitter(lim).run(is, tx, dec, enc, es, os);
     } catch (const std::exception&) {
         return -1;
     }

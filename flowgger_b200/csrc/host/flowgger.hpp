@@ -113,11 +113,18 @@ class CudaBatchDecoder {
                                   std::vector<std::string>* side_effects = nullptr) const;
     // framing + UTF-8 validation + decode of a raw byte stream on the device (fg_split_decode)
     void split_decode(const uint8_t* stream, int64_t nbytes, fg_batch_out* out, fg_framing framing = FG_FRAME_LINE);
+    // the same, but false (nothing decoded) when the stream does not fit the context: more bytes or more records
+    bool try_split_decode(const uint8_t* stream, int64_t nbytes, fg_batch_out* out, fg_framing framing);
     // decode + GelfEncoder::encode fused on the device (fg_decode_encode_gelf); `extra` = output.gelf_extra
     void decode_encode_gelf(const uint8_t* bytes, const int32_t* offsets, int32_t n,
                             const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out);
+    // framing + decode + GelfEncoder::encode fused on the device (fg_split_decode_encode_gelf); false as try_split_decode
+    bool try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
+                                      const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out,
+                                      const int32_t** line_offsets);
 
    private:
+    void set_gelf_extra(const std::vector<std::pair<std::string, std::string>>& extra);
     fg_format fmt_;
     fg_ctx* ctx_ = nullptr;
     std::mutex mu_;
@@ -223,9 +230,12 @@ class RecordBatcher {
     std::vector<int32_t> invalid_before_{0};  // "Invalid UTF-8 input" events, kept in stream order relative to the records
 };
 
-// Batched twin of LineSplitter::run (splitter/line_splitter.rs:10-54): reads lines like
-// BufRead::lines (strip "\n" and one "\r"; invalid UTF-8 => "Invalid UTF-8 input" on stderr,
-// line skipped) and feeds a RecordBatcher.
+// Batched twin of LineSplitter::run (splitter/line_splitter.rs:10-54).  It reads raw blocks of up to Limits::max_bytes
+// (at most the context's max_batch_bytes), cuts each after its last "\n" and carries the tail into the next block.  The
+// device frames the block like BufRead::lines (strip "\n" and one "\r"), checks UTF-8 (invalid => "Invalid UTF-8 input"
+// on stderr, line skipped) and decodes it (fg_split_decode_framed); with a CudaGelfEncoder and an RFC5424 decoder it also
+// encodes (fg_split_decode_encode_gelf).  A block that frames into more lines than the context holds is decoded in two
+// halves cut at a "\n" near its middle; a line longer than max_batch_bytes gets a context of its own (make_sized).
 class BatchingLineSplitter {
    public:
     struct Limits {
@@ -241,7 +251,9 @@ class BatchingLineSplitter {
    private:
     Limits lim_;
 };
-// Batched twins of NulSplitter::run (splitter/nul_splitter.rs:10-47) and SyslenSplitter::run (syslen_splitter.rs:10-57)
+// Batched twins of NulSplitter::run (splitter/nul_splitter.rs:10-47: raw blocks framed on the device, as
+// BatchingLineSplitter with NUL delimiters) and SyslenSplitter::run (syslen_splitter.rs:10-57: framed on the host, fed
+// to a RecordBatcher)
 class BatchingNulSplitter {
    public:
     BatchingNulSplitter() = default;

@@ -103,6 +103,8 @@ def load_cuda() -> C.CDLL:
         L.fg_tz_count.restype = C.c_int32
         L.fg_set_gelf_extra.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p)]
         L.fg_decode_encode_gelf.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(FgEncodedOut)]
+        L.fg_split_decode_encode_gelf.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.POINTER(FgEncodedOut),
+                                                  C.POINTER(C.POINTER(C.c_int32))]
         _cuda = L
     return _cuda
 
@@ -137,7 +139,7 @@ def load_host() -> C.CDLL:
         L.fgh_clone_decode_threads.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_int,
                                                C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_char_p, C.c_int]
         L.fgh_splitter_run_gelf.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int64, C.c_int, C.POINTER(C.c_char_p),
-                                            C.POINTER(C.c_char_p)] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 2
+                                            C.POINTER(C.c_char_p)] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 2 + [C.c_int]
         L.fgh_splitter_run.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int64, C.c_int32, C.c_int64] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         _host = L
     return _host
@@ -367,6 +369,27 @@ class BatchDecoder:
             return buf.tobytes(), offs.copy(), status.copy(), out.kernel_ms
         return buf, offs, status, out.kernel_ms
 
+    def split_decode_encode_gelf(self, stream: np.ndarray, framing: int = 0, copy: bool = True):
+        """Framing (0 = "line", 1 = "nul") + UTF-8 validation + decode + GelfEncoder::encode of a raw byte stream, all on
+        the device: (JSON bytes, int64 offsets[n+1], status uint8[n], record starts int32[n+1] in `stream` with their
+        terminators, kernel ms).  A record that is not UTF-8 has status 76 ("Invalid UTF-8 input") and an empty JSON record.
+        With copy=False the arrays are views of the context's pinned buffers (valid until the next call)."""
+        assert stream.dtype == np.uint8
+        out = FgEncodedOut()
+        lo = C.POINTER(C.c_int32)()
+        self._keep = (stream,)
+        self._check(self.L.fg_split_decode_encode_gelf(self.ctx, self.fmt, framing, _ptr(stream), len(stream), C.byref(out), C.byref(lo)),
+                    "fg_split_decode_encode_gelf")
+        n = out.n
+        offs = np.ctypeslib.as_array(out.offsets, shape=(n + 1,))
+        total = int(offs[-1]) if n else 0
+        buf = np.ctypeslib.as_array(out.bytes, shape=(max(total, 1),))[:total]
+        status = np.ctypeslib.as_array(out.status, shape=(max(n, 1),))[:n]
+        lines = np.ctypeslib.as_array(lo, shape=(n + 1,))
+        if copy:
+            return buf.tobytes(), offs.copy(), status.copy(), lines.copy(), out.kernel_ms
+        return buf, offs, status, lines, out.kernel_ms
+
     def split_decode(self, stream: np.ndarray) -> BatchResult:
         """Framing + UTF-8 validation + decode of a raw newline-terminated byte stream, all on the device."""
         assert stream.dtype == np.uint8
@@ -528,9 +551,10 @@ def clone_decode_threads(fmt: int, lines: list[bytes], nthreads: int = 2, device
 
 
 def splitter_run_gelf(dec: "BatchDecoder", text: bytes, extra: dict[str, str] | None = None, max_lines: int = 1 << 16,
-                      max_bytes: int = 16 << 20) -> tuple[bytes, bytes]:
-    """BatchingLineSplitter with input.format = rfc5424 and output.format = gelf (decode + encode fused on the GPU):
-    returns (JSON records separated by newlines, stderr text)."""
+                      max_bytes: int = 16 << 20, framing: int = 0) -> tuple[bytes, bytes]:
+    """BatchingLineSplitter (framing 0) or BatchingNulSplitter (framing 1) with input.format = rfc5424 and
+    output.format = gelf (framing, decode and encode fused on the GPU): returns (JSON records separated by newlines,
+    stderr text)."""
     H = load_host()
     ex = list((extra or {}).items())
     keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])
@@ -538,7 +562,7 @@ def splitter_run_gelf(dec: "BatchDecoder", text: bytes, extra: dict[str, str] | 
     ps = [C.c_void_p() for _ in range(2)]
     ns = [C.c_int64() for _ in range(2)]
     rc = H.fgh_splitter_run_gelf(dec._h, text, len(text), max_lines, max_bytes, len(ex), keys, vals, C.byref(ps[0]), C.byref(ns[0]),
-                                 C.byref(ps[1]), C.byref(ns[1]))
+                                 C.byref(ps[1]), C.byref(ns[1]), framing)
     if rc != 0:
         raise RuntimeError("splitter failed")
     out = []

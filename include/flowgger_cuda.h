@@ -268,6 +268,15 @@ typedef struct fg_encoded_out {
 int fg_set_gelf_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
 int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 */, const uint8_t* bytes, const int32_t* offsets, int32_t n,
                           fg_encoded_out* out);
+/* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424 decode ->
+ * GelfEncoder::encode, all on the device; only the encoded records and the record extents come back.
+ * Record i is out->bytes[out->offsets[i], out->offsets[i+1]); out->status[i] is 0, a decoder status, or the framing status
+ * whose fg_error_string is "Invalid UTF-8 input" (empty record).  *line_offsets ([n+1], starts in `stream`, each record
+ * still carrying its terminator, like fg_batch_out.line_offsets) stays valid until the next call on the context.
+ * Errors: another format or an unknown framing -> FG_E_ARG; nbytes > max_batch_bytes or more records than
+ * max_batch_lines -> FG_E_CAPACITY (the context stays usable). */
+int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 */, fg_framing framing, const uint8_t* stream,
+                                int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
 
 /* the reference's Err(&'static str) for a row status (0 -> NULL) */
 const char* fg_error_string(fg_format fmt, uint32_t status);
@@ -276,7 +285,8 @@ uint32_t fg_error_count(void);
 /* build/launch facts for tests and bench */
 const char* fg_build_info(void);          /* arch, compiler, kernel list */
 int64_t fg_kernel_launches(const fg_ctx* ctx); /* parse kernels launched by this ctx so far */
-float fg_last_split_ms(const fg_ctx* ctx);     /* device time of the framing + UTF-8 kernels of the last fg_split_decode */
+float fg_last_split_ms(const fg_ctx* ctx);     /* device time of the framing + UTF-8 kernels of the last fg_split_decode
+                                                  (or fg_split_decode_framed / fg_split_decode_encode_gelf) */
 float fg_last_dominant_kernel_ms(const fg_ctx* ctx); /* CUDA-event time of the dominant kernel alone (RFC5424: parse5424_kernel)
                                                         inside the last fg_parse_resident step */
 

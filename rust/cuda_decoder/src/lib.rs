@@ -7,7 +7,8 @@
 //!   * `Splitter<T>::run`                                                    (src/flowgger/splitter/mod.rs:18-26)
 //! All parsing happens on the GPU — including line framing, the UTF-8 check and the unescape of RFC5424 SD values; this
 //! crate hands raw blocks to `fg_split_decode` (or packed lines to `fg_decode_batch`) and materialises Records, or, for
-//! the rfc5424 -> gelf pair, forwards the records the device already encoded (`fg_decode_encode_gelf`).
+//! the rfc5424 -> gelf pair, forwards the records the device already framed, decoded and encoded
+//! (`fg_split_decode_encode_gelf`).
 #![allow(non_camel_case_types, non_upper_case_globals, dead_code)]
 
 use flowgger::flowgger::config::Config;
@@ -27,11 +28,25 @@ mod ffi {
 }
 use ffi::*;
 
+/// What `fg_create` was given apart from the capacity, kept to make a twin of a context with another capacity.
+#[derive(Clone)]
+struct CtxSpec {
+    device: i32,
+    has_schema: bool,
+    names: Vec<CString>,
+    types: Vec<i32>,
+    suffix: [Option<String>; 5],
+    tzdir: Option<CString>,
+}
+
 /// One GPU context of a fixed format (`fg_ctx`); shared by the clones handed to input threads.
 struct Ctx {
     raw: *mut fg_ctx,
     fmt: fg_format,
     suffix: [Option<String>; 5],
+    spec: CtxSpec,
+    max_bytes: usize,                        // max_batch_bytes as fg_create took it
+    extra: Option<Vec<(String, String)>>,    // the output.gelf_extra last set on the context
 }
 unsafe impl Send for Ctx {}
 impl Drop for Ctx {
@@ -86,19 +101,32 @@ impl CudaDecoder {
                 }
             }
         }
-        let name_ptrs: Vec<*const c_char> = names.iter().map(|s| s.as_ptr()).collect();
-        let sfx_c: Vec<Option<CString>> = suffix.iter().map(|s| s.as_ref().map(|x| CString::new(x.as_str()).unwrap())).collect();
+        let spec = CtxSpec {
+            device: config.lookup("input.cuda_device").and_then(|v| v.as_integer()).unwrap_or(0) as i32,
+            has_schema,
+            names,
+            types,
+            suffix,
+            tzdir: config.lookup("input.cuda_tzdir").and_then(|v| v.as_str()).map(|s| CString::new(s).unwrap()),
+        };
+        let max_bytes = config.lookup("input.cuda_max_batch_bytes").and_then(|v| v.as_integer()).unwrap_or(0);
+        let max_lines = config.lookup("input.cuda_max_batch_lines").and_then(|v| v.as_integer()).unwrap_or(0) as i32;
+        CudaDecoder::create(spec, fmt, max_bytes, max_lines)
+    }
+
+    fn create(spec: CtxSpec, fmt: fg_format, max_bytes: i64, max_lines: i32) -> CudaDecoder {
+        let name_ptrs: Vec<*const c_char> = spec.names.iter().map(|s| s.as_ptr()).collect();
+        let sfx_c: Vec<Option<CString>> = spec.suffix.iter().map(|s| s.as_ref().map(|x| CString::new(x.as_str()).unwrap())).collect();
         let mut cfg: fg_config = unsafe { std::mem::zeroed() };
-        cfg.device = config.lookup("input.cuda_device").and_then(|v| v.as_integer()).unwrap_or(0) as i32;
-        cfg.max_batch_bytes = config.lookup("input.cuda_max_batch_bytes").and_then(|v| v.as_integer()).unwrap_or(0);
-        cfg.max_batch_lines = config.lookup("input.cuda_max_batch_lines").and_then(|v| v.as_integer()).unwrap_or(0) as i32;
-        let tzdir: Option<CString> = config.lookup("input.cuda_tzdir").and_then(|v| v.as_str()).map(|s| CString::new(s).unwrap());
+        cfg.device = spec.device;
+        cfg.max_batch_bytes = max_bytes;
+        cfg.max_batch_lines = max_lines;
         cfg.rfc3164_year = 0;
-        cfg.tzdir = tzdir.as_ref().map_or(ptr::null(), |s| s.as_ptr());
-        cfg.ltsv_has_schema = has_schema as i32;
-        cfg.ltsv_schema_len = names.len() as i32;
+        cfg.tzdir = spec.tzdir.as_ref().map_or(ptr::null(), |s| s.as_ptr());
+        cfg.ltsv_has_schema = spec.has_schema as i32;
+        cfg.ltsv_schema_len = spec.names.len() as i32;
         cfg.ltsv_schema_names = name_ptrs.as_ptr();
-        cfg.ltsv_schema_types = types.as_ptr();
+        cfg.ltsv_schema_types = spec.types.as_ptr();
         for t in 1..5 {
             cfg.ltsv_suffix[t] = sfx_c[t].as_ref().map_or(ptr::null(), |s| s.as_ptr());
         }
@@ -108,7 +136,23 @@ impl CudaDecoder {
             // There is no CPU fallback: without the library + a GPU the decoder cannot exist.
             panic!("flowgger_cuda: fg_create failed ({})", rc);
         }
-        CudaDecoder { ctx: Arc::new(Mutex::new(Ctx { raw, fmt, suffix })) }
+        let max_bytes = if max_bytes > 0 { (max_bytes as usize).min(0x7FFF_FFC0) } else { 256 << 20 };  // fg_create's default and cap
+        let suffix = spec.suffix.clone();
+        CudaDecoder { ctx: Arc::new(Mutex::new(Ctx { raw, fmt, suffix, spec, max_bytes, extra: None })) }
+    }
+
+    /// max_batch_bytes of the context
+    pub fn capacity_bytes(&self) -> usize {
+        self.ctx.lock().unwrap().max_bytes
+    }
+
+    /// A context of the same format and configuration sized for `max_bytes` (one line longer than a whole batch).
+    pub fn make_sized(&self, max_bytes: usize) -> CudaDecoder {
+        let (spec, fmt) = {
+            let c = self.ctx.lock().unwrap();
+            (c.spec.clone(), c.fmt)
+        };
+        CudaDecoder::create(spec, fmt, max_bytes as i64, 64)
     }
 
     /// Decode `n` lines packed as bytes + offsets; calls `f(i, result)` in input order.
@@ -129,27 +173,144 @@ impl CudaDecoder {
     }
 }
 
+/// Extent of line i of a raw stream framed on the device without its terminator (BufRead::lines: the '\n' and one '\r'
+/// before it)
+fn line_extent(stream: &[u8], line_offsets: &[i32], i: usize) -> (usize, usize) {
+    let (lo, mut hi) = (line_offsets[i] as usize, line_offsets[i + 1] as usize);
+    if hi > lo && stream[hi - 1] == b'\n' { hi -= 1; if hi > lo && stream[hi - 1] == b'\r' { hi -= 1; } }
+    (lo, hi)
+}
+
+/// The reference's `&'static str` for a status
+fn error_str(fmt: fg_format, status: u32) -> &'static str {
+    unsafe {
+        let s = CStr::from_ptr(fg_error_string(fmt, status));
+        std::str::from_utf8_unchecked(std::slice::from_raw_parts(s.as_ptr() as *const u8, s.to_bytes().len()))
+    }
+}
+
 impl CudaDecoder {
     /// Framing + UTF-8 validation + decode of a raw stream on the device (`fg_split_decode`): `f(i, line, result)` in
     /// stream order; a line that is not UTF-8 arrives as `Err("Invalid UTF-8 input")` (line_splitter.rs:22-25).
-    pub fn split_decode<F: FnMut(usize, &[u8], Result<Record, &'static str>, &[String])>(&self, stream: &[u8], mut f: F) {
+    /// false (nothing decoded) when the stream does not fit the context: more bytes or more lines than it holds.
+    pub fn split_decode<F: FnMut(usize, &[u8], Result<Record, &'static str>, &[String])>(&self, stream: &[u8], mut f: F) -> bool {
         let ctx = self.ctx.lock().unwrap();
         let mut out: fg_batch_out = unsafe { std::mem::zeroed() };
         let rc = unsafe { fg_split_decode(ctx.raw, ctx.fmt, stream.as_ptr(), stream.len() as i64, &mut out) };
+        if rc == FG_E_CAPACITY {
+            return false;
+        }
         if rc != 0 {
             let e = unsafe { CStr::from_ptr(fg_last_error(ctx.raw)) }.to_string_lossy().into_owned();
             panic!("fg_split_decode: {}", e);
         }
         let offs = unsafe { std::slice::from_raw_parts(out.line_offsets, out.n as usize + 1) };
         for i in 0..out.n as usize {
-            // BufRead::lines: drop the '\n' and one '\r' before it
-            let (lo, mut hi) = (offs[i] as usize, offs[i + 1] as usize);
-            if hi > lo && stream[hi - 1] == b'\n' { hi -= 1; if hi > lo && stream[hi - 1] == b'\r' { hi -= 1; } }
-            let ext = [lo as i32, hi as i32];
+            let (lo, hi) = line_extent(stream, offs, i);
             let mut side = Vec::new();
             // `materialize` reads the extent of line i from offsets[i..i+2]: hand it the stripped extent
-            let r = materialize_ext(&ctx, &out, stream, ext[0], ext[1], i, &mut side);
+            let r = materialize_ext(&ctx, &out, stream, lo as i32, hi as i32, i, &mut side);
             f(i, &stream[lo..hi], r, &side);
+        }
+        true
+    }
+
+    /// Framing + UTF-8 validation + decode + `GelfEncoder::encode` of a raw stream on the device
+    /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424"): `f(line, Ok(json) | Err(error))` in stream order, `line`
+    /// without its terminator.  false (nothing decoded) when the stream does not fit the context.
+    pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>)>(&self, stream: &[u8], extra: &[(String, String)],
+                                                                                   mut f: F) -> bool {
+        let mut ctx = self.ctx.lock().unwrap();
+        if ctx.extra.as_deref() != Some(extra) {
+            let keys: Vec<CString> = extra.iter().map(|(k, _)| CString::new(k.as_str()).unwrap()).collect();
+            let vals: Vec<CString> = extra.iter().map(|(_, v)| CString::new(v.as_str()).unwrap()).collect();
+            let kp: Vec<*const c_char> = keys.iter().map(|s| s.as_ptr()).collect();
+            let vp: Vec<*const c_char> = vals.iter().map(|s| s.as_ptr()).collect();
+            assert_eq!(unsafe { fg_set_gelf_extra(ctx.raw, kp.len() as i32, kp.as_ptr(), vp.as_ptr()) }, 0);
+            ctx.extra = Some(extra.to_vec());
+        }
+        let mut out: fg_encoded_out = unsafe { std::mem::zeroed() };
+        let mut lines: *const i32 = ptr::null();
+        let rc = unsafe {
+            fg_split_decode_encode_gelf(ctx.raw, ctx.fmt, fg_framing_FG_FRAME_LINE, stream.as_ptr(), stream.len() as i64, &mut out,
+                                        &mut lines)
+        };
+        if rc == FG_E_CAPACITY {
+            return false;
+        }
+        if rc != 0 {
+            let e = unsafe { CStr::from_ptr(fg_last_error(ctx.raw)) }.to_string_lossy().into_owned();
+            panic!("fg_split_decode_encode_gelf: {}", e);
+        }
+        let n = out.n as usize;
+        let offs = unsafe { std::slice::from_raw_parts(lines, n + 1) };
+        for i in 0..n {
+            let (lo, hi) = line_extent(stream, offs, i);
+            let (st, a, b) = unsafe { (*out.status.add(i), *out.offsets.add(i) as usize, *out.offsets.add(i + 1) as usize) };
+            if st == 0 {
+                f(&stream[lo..hi], Ok(unsafe { std::slice::from_raw_parts(out.bytes.add(a), b - a) }));
+            } else {
+                f(&stream[lo..hi], Err(error_str(ctx.fmt, st as u32)));
+            }
+        }
+        true
+    }
+}
+
+/// The lines of `block` in stream order through `run`, which returns false when they do not fit the context it is given:
+/// such a block is decoded in two halves cut after a '\n' near its middle, and a lone line longer than the context's
+/// max_batch_bytes on a context of its own, sized for it (rare, slow, correct: the reference takes lines of any length).
+fn decode_fitting<F: FnMut(&CudaDecoder, &[u8]) -> bool>(gpu: &CudaDecoder, block: &[u8], run: &mut F) {
+    let n = block.len();
+    if n == 0 || (n <= gpu.capacity_bytes() && run(gpu, block)) {
+        return;
+    }
+    let mid = n / 2;
+    // the last byte ends the last line: it is no cut
+    let cut = block[mid..n - 1].iter().position(|&c| c == b'\n').map(|p| mid + p + 1)
+        .or_else(|| block[..mid].iter().rposition(|&c| c == b'\n').map(|p| p + 1));
+    match cut {
+        Some(c) => {
+            decode_fitting(gpu, &block[..c], run);
+            decode_fitting(gpu, &block[c..], run);
+        }
+        None => {
+            let big = gpu.make_sized(n + 4096);
+            assert!(run(&big, block), "a line does not fit a context sized for it");
+        }
+    }
+}
+
+/// Reads RAW BLOCKS of `max_bytes` or more (no per-line `String`), cuts each block after its last '\n' and hands the
+/// whole lines to `flush`, keeping the unterminated tail for the next block; at EOF the rest, an unterminated last line
+/// included.
+fn run_blocks<T: Read, F: FnMut(&[u8])>(mut buf_reader: BufReader<T>, max_bytes: usize, mut flush: F) {
+    let mut block: Vec<u8> = Vec::with_capacity(max_bytes);
+    loop {
+        let got = match buf_reader.fill_buf() {
+            Ok(b) => { let n = b.len(); block.extend_from_slice(b); n }
+            Err(e) => match e.kind() {
+                ErrorKind::Interrupted => continue,
+                ErrorKind::WouldBlock => {
+                    flush(&block);
+                    let _ = writeln!(stderr(), "Client hasn't sent any data for a while - Closing idle connection");
+                    return;
+                }
+                _ => { flush(&block); return; }
+            },
+        };
+        buf_reader.consume(got);
+        if got == 0 {                       // EOF: an unterminated last line is still a line
+            flush(&block);
+            return;
+        }
+        if block.len() >= max_bytes {
+            // decode every complete line of the block, keep the unterminated tail for the next one
+            let cut = block.iter().rposition(|&c| c == b'\n').map_or(0, |p| p + 1);
+            if cut > 0 {
+                flush(&block[..cut]);
+                block.drain(..cut);
+            }
         }
     }
 }
@@ -369,7 +530,8 @@ impl Decoder for CudaDecoder {
 /// Batched twin of `LineSplitter` (src/flowgger/splitter/line_splitter.rs:10-54): inserted between `input` and
 /// `decoder`.  It reads RAW BLOCKS (no per-line `String`), cuts each block after its last '\n' and hands the block to
 /// `fg_split_decode`: line framing (`BufRead::lines`: "\n", one "\r"), the UTF-8 check of `String` and the decode all run
-/// on the device; stderr text and record order are those of the reference.
+/// on the device; stderr text and record order are those of the reference.  A block that holds more lines than the
+/// context is decoded in halves, and a line longer than the context's max_batch_bytes on a context sized for it.
 pub struct BatchingLineSplitter {
     pub gpu: CudaDecoder,
     pub max_bytes: usize,
@@ -377,105 +539,47 @@ pub struct BatchingLineSplitter {
 
 impl BatchingLineSplitter {
     fn flush<F: FnMut(Vec<u8>)>(&self, block: &[u8], encoder: &Box<dyn Encoder>, send: &mut F) {
-        self.gpu.split_decode(block, |_, line, r, side| {
-            for s in side { println!("{}", s); }
-            match r.and_then(|rec| encoder.encode(rec)) {
-                Ok(bytes) => send(bytes),
-                Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
-                Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
-            }
+        decode_fitting(&self.gpu, block, &mut |gpu: &CudaDecoder, part: &[u8]| {
+            gpu.split_decode(part, |_, line, r, side| {
+                for s in side { println!("{}", s); }
+                match r.and_then(|rec| encoder.encode(rec)) {
+                    Ok(bytes) => send(bytes),
+                    Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
+                    Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
+                }
+            })
         });
     }
 }
 
 impl<T: Read> Splitter<T> for BatchingLineSplitter {
-    fn run(&self, mut buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, encoder: Box<dyn Encoder>) {
-        let mut block: Vec<u8> = Vec::with_capacity(self.max_bytes);
+    fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, encoder: Box<dyn Encoder>) {
         let mut send = |bytes: Vec<u8>| tx.send(bytes).unwrap();
-        loop {
-            let got = match buf_reader.fill_buf() {
-                Ok(b) => { let n = b.len(); block.extend_from_slice(b); n }
-                Err(e) => match e.kind() {
-                    ErrorKind::Interrupted => continue,
-                    ErrorKind::WouldBlock => {
-                        self.flush(&block, &encoder, &mut send);
-                        let _ = writeln!(stderr(), "Client hasn't sent any data for a while - Closing idle connection");
-                        return;
-                    }
-                    _ => { self.flush(&block, &encoder, &mut send); return; }
-                },
-            };
-            buf_reader.consume(got);
-            if got == 0 {                       // EOF: an unterminated last line is still a line
-                self.flush(&block, &encoder, &mut send);
-                return;
-            }
-            if block.len() >= self.max_bytes {
-                // decode every complete line of the block, keep the unterminated tail for the next one
-                let cut = block.iter().rposition(|&c| c == b'\n').map_or(0, |p| p + 1);
-                if cut > 0 {
-                    self.flush(&block[..cut], &encoder, &mut send);
-                    block.drain(..cut);
-                }
-            }
-        }
+        let max_bytes = self.max_bytes.min(self.gpu.capacity_bytes());
+        run_blocks(buf_reader, max_bytes, |block| self.flush(block, &encoder, &mut send));
     }
 }
 
-/// `output.format = "gelf"` with `input.format = "rfc5424"`: decode AND encode run on the device
-/// (`fg_decode_encode_gelf`, replaces Decoder::decode + GelfEncoder::encode of line_splitter.rs:50-52); only the encoded
-/// records come back.  Lines are framed on the host here (the fused entry point takes offsets).
+/// `output.format = "gelf"` with `input.format = "rfc5424"`: framing, the UTF-8 check, decode AND encode run on the device
+/// (`fg_split_decode_encode_gelf`, replaces BufRead::lines + Decoder::decode + GelfEncoder::encode of
+/// line_splitter.rs:17-52); it reads raw blocks like `BatchingLineSplitter` and only the encoded records come back.
 pub struct FusedGelfLineSplitter {
     pub gpu: CudaDecoder,
     pub extra: Vec<(String, String)>,   // output.gelf_extra (gelf_encoder.rs:29-48)
-    pub max_lines: usize,
     pub max_bytes: usize,
 }
 
 impl<T: Read> Splitter<T> for FusedGelfLineSplitter {
     fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
-        let ctx = self.gpu.ctx.lock().unwrap();
-        let keys: Vec<CString> = self.extra.iter().map(|(k, _)| CString::new(k.as_str()).unwrap()).collect();
-        let vals: Vec<CString> = self.extra.iter().map(|(_, v)| CString::new(v.as_str()).unwrap()).collect();
-        let kp: Vec<*const c_char> = keys.iter().map(|s| s.as_ptr()).collect();
-        let vp: Vec<*const c_char> = vals.iter().map(|s| s.as_ptr()).collect();
-        assert_eq!(unsafe { fg_set_gelf_extra(ctx.raw, kp.len() as i32, kp.as_ptr(), vp.as_ptr()) }, 0);
-        let mut arena: Vec<u8> = Vec::with_capacity(self.max_bytes);
-        let mut offsets: Vec<i32> = vec![0];
-        let flush = |arena: &mut Vec<u8>, offsets: &mut Vec<i32>| {
-            if offsets.len() > 1 {
-                let mut out: fg_encoded_out = unsafe { std::mem::zeroed() };
-                let rc = unsafe { fg_decode_encode_gelf(ctx.raw, ctx.fmt, arena.as_ptr(), offsets.as_ptr(), offsets.len() as i32 - 1, &mut out) };
-                assert_eq!(rc, 0);
-                for i in 0..out.n as usize {
-                    let (st, lo, hi) = unsafe { (*out.status.add(i), *out.offsets.add(i) as usize, *out.offsets.add(i + 1) as usize) };
-                    if st == 0 {
-                        tx.send(unsafe { std::slice::from_raw_parts(out.bytes.add(lo), hi - lo) }.to_vec()).unwrap();
-                    } else {
-                        let e = unsafe { CStr::from_ptr(fg_error_string(ctx.fmt, st as u32)) }.to_string_lossy();
-                        let line = String::from_utf8_lossy(&arena[offsets[i] as usize..offsets[i + 1] as usize]);
-                        let _ = writeln!(stderr(), "{}: [{}]", e, line.trim());
-                    }
-                }
-            }
-            arena.clear();
-            offsets.clear();
-            offsets.push(0);
-        };
-        for line in buf_reader.lines() {
-            match line {
-                Ok(line) => {
-                    if arena.len() + line.len() > self.max_bytes || offsets.len() > self.max_lines { flush(&mut arena, &mut offsets); }
-                    arena.extend_from_slice(line.as_bytes());
-                    offsets.push(arena.len() as i32);
-                }
-                Err(e) => match e.kind() {
-                    ErrorKind::Interrupted => continue,
-                    ErrorKind::InvalidInput | ErrorKind::InvalidData => { flush(&mut arena, &mut offsets); let _ = writeln!(stderr(), "Invalid UTF-8 input"); }
-                    _ => break,
-                },
-            }
-        }
-        flush(&mut arena, &mut offsets);
+        let max_bytes = self.max_bytes.min(self.gpu.capacity_bytes());
+        run_blocks(buf_reader, max_bytes, |block| {
+            decode_fitting(&self.gpu, block, &mut |gpu: &CudaDecoder, part: &[u8]| {
+                gpu.split_decode_encode_gelf(part, &self.extra, |line, r| match r {
+                    Ok(json) => tx.send(json.to_vec()).unwrap(),
+                    Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
+                    Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
+                })
+            })
+        });
     }
 }

@@ -1,0 +1,152 @@
+"""Framing on the device vs on the host for the default pipeline (input.format = "rfc5424", output.format = "gelf").
+
+    python tools/bench_split_encode.py [--lines 10000000] [--steps 10] [--warmup 2] [--splitter-gb 1.0] [--splitter-only]
+
+On the C2 RFC5424 workload of bench.py (seed 5424, the same mean line length), joined with '\\n' in pinned memory:
+  1. fg_split_decode_encode_gelf on the raw stream and fg_decode_encode_gelf on the same lines framed beforehand, timed
+     alternately after warm-ups; both must return byte-identical records and statuses;
+  2. the C++ BatchingLineSplitter with the fused GELF encoder end to end over at least --splitter-gb of the same text
+     (text in, every JSON record handed to the sender, stderr captured).
+Prints one JSON line per section, with the card's name and power limit.  --splitter-only runs section 2 alone."""
+from __future__ import annotations
+
+import argparse
+import json
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+REPO = Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(REPO))
+
+import flowgger_b200 as fb  # noqa: E402
+
+SEED, MEAN = 5424, 169.2  # bench.py: SEEDS["rfc5424"], GEN_MEAN["rfc5424"]
+
+
+def card() -> dict:
+    try:
+        q = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power, clk = [x.strip() for x in q.split(",")]
+        return {"gpu": name, "power_limit": power, "sm_clock_max": clk}
+    except Exception as e:  # noqa: BLE001
+        return {"gpu": None, "error": str(e)}
+
+
+def workload(n: int) -> tuple[np.ndarray, np.ndarray]:
+    """the raw stream (every line followed by '\\n') and its line offsets, terminators included"""
+    return fb.generate(fb.FMT_RFC5424, SEED, n, mean_len=MEAN, bad_frac=0.005, nthreads=32, terminated=True)
+
+
+def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> None:
+    n = len(soffs) - 1
+    keep = stream != ord("\n")  # the generator puts no '\n' inside a line
+    lines = stream[keep]
+    loffs = (soffs - np.arange(n + 1, dtype=np.int64)).astype(np.int32)
+    del keep
+    split = fb.BatchDecoder(fb.FMT_RFC5424, max_batch_bytes=len(stream) + (1 << 20), max_batch_lines=n + 64)
+    pre = fb.BatchDecoder(fb.FMT_RFC5424, max_batch_bytes=len(stream) + (1 << 20), max_batch_lines=n + 64)
+    try:
+        hs = split.host_alloc(len(stream))
+        hs[:] = stream
+        hl = pre.host_alloc(len(lines))
+        hl[:] = lines
+        ho = pre.host_alloc(loffs.nbytes, dtype=np.int32)
+        ho[:] = loffs
+        del lines
+        for _ in range(args.warmup):
+            split.split_decode_encode_gelf(hs, copy=False)
+            pre.decode_encode_gelf(hl, ho, copy=False)
+        t = {"split": [], "pre": []}
+        k = {"split": [], "pre": []}
+        framing_ms = []
+        for _ in range(args.steps):
+            t0 = time.perf_counter()
+            _, _, _, _, km = split.split_decode_encode_gelf(hs, copy=False)
+            t["split"].append(time.perf_counter() - t0)
+            k["split"].append(km)
+            framing_ms.append(split.last_split_ms())
+            t0 = time.perf_counter()
+            _, _, _, km = pre.decode_encode_gelf(hl, ho, copy=False)
+            t["pre"].append(time.perf_counter() - t0)
+            k["pre"].append(km)
+        sb, so, ss, sl, _ = split.split_decode_encode_gelf(hs, copy=False)
+        pb, po, ps, _ = pre.decode_encode_gelf(hl, ho, copy=False)
+        assert len(ss) == n and np.array_equal(sl, soffs), "the device framed other lines than the generator made"
+        assert np.array_equal(so, po) and np.array_equal(ss, ps) and np.array_equal(sb, pb), \
+            "fg_split_decode_encode_gelf and fg_decode_encode_gelf disagree"
+        out_bytes = int(so[-1])
+        for key, api, in_bytes in (("split", "fg_split_decode_encode_gelf (pinned raw stream in)", len(stream)),
+                                   ("pre", "fg_decode_encode_gelf (pinned lines + int32 offsets in, framed beforehand)",
+                                    int(loffs[-1]) + loffs.nbytes)):
+            med = float(np.median(t[key]))
+            rec = {"section": key, "api": api, "lines": n, "input_bytes": in_bytes, "json_bytes": out_bytes,
+                   "records": int((ss == 0).sum()), "steps": args.steps, "call_ms_median": med * 1e3,
+                   "call_ms_min": min(t[key]) * 1e3, "call_ms_max": max(t[key]) * 1e3,
+                   "lines_per_s": n / med, "input_gb_per_s": in_bytes / med / 1e9, "output_gb_per_s": out_bytes / med / 1e9,
+                   "kernel_ms_median": float(np.median(k[key])), **info}
+            if key == "split":
+                rec["framing_stage_ms_median"] = float(np.median(framing_ms))
+            print(json.dumps(rec), flush=True)
+    finally:
+        split.close()
+        pre.close()
+
+
+def splitter(args, stream: np.ndarray, info: dict) -> None:
+    # pieces of ~400 MB of whole lines: the records of one call come back as one Python bytes object, which ctypes
+    # copies with an int length (< 2 GiB), and the JSON is about 2.6 times the text
+    piece = 400_000_000
+    cuts = [0]
+    while cuts[-1] < len(stream):
+        end = min(len(stream), cuts[-1] + piece)
+        cuts.append(cuts[-1] + int(np.flatnonzero(stream[cuts[-1]:end] == ord("\n"))[-1]) + 1 if end < len(stream) else end)
+    texts = [stream[a:b].tobytes() for a, b in zip(cuts[:-1], cuts[1:])]
+    want = int(args.splitter_gb * 1e9)
+    dec = fb.BatchDecoder(fb.FMT_RFC5424, max_batch_bytes=64 << 20, max_batch_lines=1 << 20)
+    wall, in_bytes, json_bytes, lines, n_rec, n_err = 0.0, 0, 0, 0, 0, 0
+    try:
+        small = texts[0][: 1 << 20]
+        fb.splitter_run_gelf(dec, small[: small.rindex(b"\n") + 1], max_lines=1 << 19, max_bytes=64 << 20)  # warm-up
+        k = 0
+        while in_bytes < want:
+            text = texts[k % len(texts)]
+            k += 1
+            t0 = time.perf_counter()
+            records, err = fb.splitter_run_gelf(dec, text, max_lines=1 << 19, max_bytes=64 << 20)
+            wall += time.perf_counter() - t0
+            r, e, t = records.count(b"\n"), err.count(b"\n"), text.count(b"\n")
+            assert r + e == t, (r, e, t)
+            n_rec, n_err, lines = n_rec + r, n_err + e, lines + t
+            in_bytes += len(text)
+            json_bytes += len(records) - r
+    finally:
+        dec.close()
+    print(json.dumps({"section": "splitter", "api": "BatchingLineSplitter + CudaGelfEncoder (fgh_splitter_run_gelf: text in, "
+                      "records + stderr out, 64 MiB batches; wall time summed over calls of ~400 MB)", "calls": k,
+                      "lines": lines, "input_bytes": in_bytes, "json_bytes": json_bytes, "records": n_rec, "stderr_lines": n_err,
+                      "wall_s": wall, "lines_per_s": lines / wall, "input_gb_per_s": in_bytes / wall / 1e9,
+                      "output_gb_per_s": json_bytes / wall / 1e9, **info}), flush=True)
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--lines", type=int, default=10_000_000)
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--splitter-gb", type=float, default=1.0)
+    ap.add_argument("--splitter-only", action="store_true")
+    args = ap.parse_args()
+    info = card()
+    stream, soffs = workload(args.lines)
+    if not args.splitter_only:
+        device_paths(args, stream, soffs, info)
+    splitter(args, stream, info)
+
+
+if __name__ == "__main__":
+    main()
