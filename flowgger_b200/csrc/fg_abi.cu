@@ -566,13 +566,25 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
     return FG_OK;
 }
 
-// The fused GELF encoder over the RFC5424 results of lines [l0, l0 + n), parse step k
-int launch_encode(fg_ctx* c, int k, int l0, int n, int tile, cudaStream_t s) {
-    fg::GelfEncodeParams E;
+// The decoders whose device-resident results the fused GELF encoder reads
+bool gelf_fusable(int fmt) { return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164; }
+
+// The fused GELF encoder over the decoder's results of lines [l0, l0 + n), parse step k
+int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream_t s) {
+    fg::GelfEncodeParams E{};
     E.bytes = c->bytes.d;
     E.offsets = c->offsets.d + l0;
     E.n = n;
-    E.rows = reinterpret_cast<const uint4*>(c->rows5.d + l0);
+    if (fmt == FG_FMT_RFC5424) {
+        E.rows = reinterpret_cast<const uint4*>(c->rows5.d + l0);
+    } else {
+        const uint8_t* r = c->rows.d;
+        E.r3_ts = (const double*)(r + col_off(c, C_TS)) + l0;
+        E.r3_meta = (const uint32_t*)(r + col_off(c, C_META)) + l0;
+        E.r3_host = (const int2*)(r + col_off(c, C_HOST)) + l0;
+        E.r3_msg = (const int2*)(r + col_off(c, C_MSG)) + l0;
+        E.r3_full = (const int2*)(r + col_off(c, C_FULL)) + l0;
+    }
     E.entries = dev<unsigned long long>(c, T_E8);
     E.arena = dev<uint8_t>(c, T_ARENA);
     E.wide_rows = dev<fg::WideRow>(c, T_WIDE);
@@ -595,8 +607,10 @@ int launch_encode(fg_ctx* c, int k, int l0, int n, int tile, cudaStream_t s) {
     E.entry_cap = cap32(c, T_E8);
     E.wide_cap = cap32(c, T_WIDE);
     E.wentry_cap = cap32(c, T_ENTRIES);
-    E.tile_bytes = std::min(4 * tile, c->max_tile5);  // the encoder's CTAs take 256 lines (4 x the parse kernel's 64)
-    FG_CUDA(c, fg::launch_gelf_encode(E, c->scan_temp.d, c->scan_temp_bytes, s));
+    E.arena_cap = cap32(c, T_ARENA);
+    // the encoder's CTAs take 256 lines (4 x the parse kernel's 64); configure_gelf_encode allowed max_tile5
+    E.tile_bytes = std::min(4 * tile, c->max_tile5);
+    FG_CUDA(c, fg::launch_gelf_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
     c->launches += 4;
     return FG_OK;
 }
@@ -756,7 +770,7 @@ int parse_step(fg_ctx* c, int fmt, int k, int l0, int n, int tile, const uint8_t
     FG_CUDA(c, cudaEventRecord(e.k0, s));
     if (int rc = launch_lines(c, fmt, l0, n, tile, invalid, strip, s)) return rc;
     if (encode)
-        if (int rc = launch_encode(c, k, l0, n, tile, s)) return rc;
+        if (int rc = launch_encode(c, fmt, k, l0, n, tile, s)) return rc;
     FG_CUDA(c, cudaEventRecord(e.k1, s));
     FG_CUDA(c, cudaMemcpyAsync(c->counts.h + (size_t)k * fg::K5_COUNT, c->k.d, kCountBytes, cudaMemcpyDeviceToHost, s));
     if (encode)
@@ -1162,12 +1176,12 @@ int fg_set_gelf_extra(fg_ctx* c, int32_t n, const char* const* keys, const char*
     return build_static_items(c);
 }
 
-// decode (RFC5424) + GelfEncoder::encode fused: H2D lines -> parse kernels -> size / scan / write kernels -> D2H of the
-// encoded records only, chunk by chunk; the decoder's rows and side tables never leave the device.
+// decode (RFC5424 or RFC3164) + GelfEncoder::encode fused: H2D lines -> parse kernels -> size / scan / write kernels ->
+// D2H of the encoded records only, chunk by chunk; the decoder's rows and side tables never leave the device.
 int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
     if (!c || !out) return FG_E_ARG;
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
-    if (fmt != FG_FMT_RFC5424) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
+    if (!gelf_fusable((int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
     if (int rc = begin_call(c, fmt)) return rc;
     const int C = c->chunk_lines;
     const int chunks = n > 0 ? (n + C - 1) / C : 1;
@@ -1358,11 +1372,12 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
     return FG_OK;
 }
 
-// framing + decode (RFC5424) + GelfEncoder::encode on the device: only the encoded records and the line offsets come back
+// framing + decode (RFC5424 or RFC3164) + GelfEncoder::encode on the device: only the encoded records and the line
+// offsets come back
 int fg_split_decode_encode_gelf(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
                                 const int32_t** line_offsets) {
     if (!c || !out || !line_offsets) return FG_E_ARG;
-    if (fmt != FG_FMT_RFC5424) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
+    if (!gelf_fusable((int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
     int32_t n;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;

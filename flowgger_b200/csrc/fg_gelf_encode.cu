@@ -6,8 +6,12 @@
 // an earlier one (SD pairs replace fixed fields, output.gelf_extra replaces everything), compact separators, strings
 // with `"` `\\` \b \f \n \r \t escaped, Record.ts through dtoa (fg_dtoa.cuh).
 //
-// Input = the decoder's device-resident results (compact rows + 8-byte entries + arena, or wide rows); nothing of them
-// travels to the host in this mode.  Launches per chunk of lines:
+// Input = the decoder's device-resident results; nothing of them travels to the host in this mode.  Two record sources,
+// chosen at compile time (the kernels are templates on the source, everything after the record view is shared):
+//   From5424  compact rows + 8-byte entries + arena, or wide rows (structured data; every fixed field present)
+//   From3164  the row columns of parse3164_kernel + the arena of re-joined messages (rfc3164_decoder.rs:71-82, 106-117:
+//             no appname, procid or structured data; no severity without <PRI>; msg always Some, possibly "")
+// Launches per chunk of lines:
 //   gelf_size_kernel   one thread per line: exact length of its record (0 for a line the decoder rejected); the bytes of
 //                      the CTA's 256 lines are staged in shared memory by one TMA bulk copy and handed to the threads
 //                      in order of line length (both kernels)
@@ -170,6 +174,43 @@ __device__ __forceinline__ void load_view(const GelfEncodeParams& P, const ByteS
     }
 }
 
+constexpr uint32_t kMsgArena = 0x40u;    // FG_FLAG_MSG_ARENA: msg.x indexes the arena
+constexpr uint32_t kNoSeverity = 0xFFu;  // a line without <PRI>: Record.severity is None
+
+// An RFC3164 row: absolute spans (fg_parse3164.cu).  msg is never None: an empty message still gets a non-null pointer.
+__device__ __forceinline__ void load_view_3164(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) {
+    const uint32_t meta = P.r3_meta[i];
+    r.ok = (meta & 0xFFu) == 0u;
+    r.wide = false;
+    r.has_sd = false;
+    r.first = r.count = 0;
+    if (!r.ok) return;
+    r.severity = (meta >> 16) & 0xFFu;
+    r.ts = P.r3_ts[i];
+    const int2 h = P.r3_host[i], m = P.r3_msg[i], f = P.r3_full[i];
+    r.host = Span{B.at(h.x), h.y};
+    r.full = Span{B.at(f.x), f.y};
+    if ((meta >> 24) & kMsgArena) {
+        if ((unsigned long long)(uint32_t)m.x + (uint32_t)m.y > (unsigned long long)P.arena_cap) { r.ok = false; return; }
+        r.msg = Span{P.arena + (uint32_t)m.x, m.y};
+    } else {
+        r.msg = Span{B.at(m.x), m.y};
+    }
+}
+
+// The record sources the kernels are instantiated for.  kSd: the record may carry structured data.  kOptional:
+// application_name and process_id are None, and level is None without a severity.
+struct From5424 {
+    static constexpr bool kSd = true, kOptional = false;
+    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view(P, B, i, r); }
+    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.rows[2 * (size_t)i].z & 0xFFu; }
+};
+struct From3164 {
+    static constexpr bool kSd = false, kOptional = true;
+    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_3164(P, B, i, r); }
+    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.r3_meta[i] & 0xFFu; }
+};
+
 // pair e of the line (false: the row is an element header)
 __device__ __forceinline__ bool load_pair(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, uint32_t e, Span& name,
                                           Span& val) {
@@ -319,14 +360,15 @@ struct PairCursor {
 // every record, so the lanes of a warp stay on the same item (the first version merged pair by pair per lane: the lanes
 // drifted apart by their pair counts and every static item ran a few lanes wide); the SD pairs that
 // sort before the current item are emitted by an inner loop whose trip count is the warp's maximum.
+template <class Src>
 __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, bool live, uint8_t* num,
                                                SegList& L) {
     if (live) L.lit(L_OPEN, 1);
     bool first = true;
     PairCursor pc;
-    if (live) pc.init(P, B, r);
+    if (Src::kSd && live) pc.init(P, B, r);
     Span bn{nullptr, 0}, bv{nullptr, 0};
-    bool have = live && pc.next(P, B, r, bn, bv);
+    bool have = Src::kSd && live && pc.next(P, B, r, bn, bv);
     for (int si = 0; si <= P.n_static; ++si) {  // warp-uniform; si == n_static: the pairs after the last static item
         const bool tail = si == P.n_static;
         Span key{nullptr, 0};
@@ -360,6 +402,7 @@ __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const 
                 }
             }
             if (kind == GF_SDID && !r.has_sd) take = false;
+            if (Src::kOptional && (kind == GF_APP || kind == GF_PROC || (kind == GF_LEVEL && r.severity == kNoSeverity))) take = false;
             if (take) {
                 // the literal is `,"key":` (for an extra `,"key":"value"`): the comma is skipped for the first item
                 const uint8_t* lit = P.static_blob + P.static_lit_off[si];
@@ -459,14 +502,14 @@ __device__ __forceinline__ void run_segments(const SegList& L, bool live, Sink& 
 }
 
 // a record of any size: windows of kMaxSegs segments, every window through the warp-uniform loop
-template <class Sink>
+template <class Src, class Sink>
 __device__ __forceinline__ void emit_record(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, bool live, Sink& s) {
     uint8_t num[32];
     SegList L;
     int skip = 0;
     for (;;) {
         L.reset(skip);
-        build_segments(P, B, r, live, num, L);
+        build_segments<Src>(P, B, r, live, num, L);
         run_segments(L, live, s);
         skip += kMaxSegs;
         if (!__any_sync(0xFFFFFFFFu, live && L.idx > skip)) break;
@@ -539,6 +582,7 @@ __device__ __forceinline__ int sorted_line(const GelfEncodeParams& P, EncShared&
     return tid < last - first ? first + (int)sh.perm[tid] : -1;
 }
 
+template <class Src>
 __global__ void __launch_bounds__(kEncLines) gelf_size_kernel(const __grid_constant__ GelfEncodeParams P) {
     extern __shared__ __align__(128) uint8_t tile[];
     __shared__ __align__(8) EncShared sh;
@@ -549,12 +593,12 @@ __global__ void __launch_bounds__(kEncLines) gelf_size_kernel(const __grid_const
     const bool valid = i >= 0;
     RecView r;
     r.ok = false;
-    if (valid) load_view(P, B, i, r);
+    if (valid) Src::load(P, B, i, r);
     CountSink s;
-    emit_record(P, B, r, r.ok, s);
+    emit_record<Src>(P, B, r, r.ok, s);
     if (!valid) return;
     P.lens[i] = r.ok ? s.n : 0u;
-    P.status[i] = (uint8_t)(P.rows[2 * (size_t)i].z & 0xFFu);
+    P.status[i] = (uint8_t)Src::status(P, i);
 }
 
 // chunk totals: base[k + 1] = base[k] + bytes of this chunk (one thread)
@@ -564,6 +608,7 @@ __global__ void gelf_base_kernel(const __grid_constant__ GelfEncodeParams P) {
     P.base[1] = P.base[0] + total;
 }
 
+template <class Src>
 __global__ void __launch_bounds__(kEncLines) gelf_write_kernel(const __grid_constant__ GelfEncodeParams P) {
     extern __shared__ __align__(128) uint8_t tile[];
     __shared__ __align__(8) EncShared sh;
@@ -584,17 +629,36 @@ __global__ void __launch_bounds__(kEncLines) gelf_write_kernel(const __grid_cons
     const bool live = valid && len != 0u && at + len <= P.out_cap;
     RecView r;
     r.ok = false;
-    if (live) load_view(P, B, i, r);
+    if (live) Src::load(P, B, i, r);
     WordSink s(P.out + at);
-    emit_record(P, B, r, live && r.ok, s);
+    emit_record<Src>(P, B, r, live && r.ok, s);
+}
+
+template <class Src>
+cudaError_t configure_src(int max_tile_bytes) {
+    cudaError_t e = cudaFuncSetAttribute(gelf_size_kernel<Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_tile_bytes);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(gelf_write_kernel<Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_tile_bytes);
+}
+
+template <class Src>
+cudaError_t launch_src(const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream) {
+    const int grid = (p.n + kEncLines - 1) / kEncLines;
+    gelf_size_kernel<Src><<<grid, kEncLines, p.tile_bytes, stream>>>(p);
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(d_scan_temp, scan_temp_bytes, p.lens, p.rel, p.n, stream);
+    if (e != cudaSuccess) return e;
+    gelf_base_kernel<<<1, 1, 0, stream>>>(p);
+    gelf_write_kernel<Src><<<grid, kEncLines, p.tile_bytes, stream>>>(p);
+    return cudaGetLastError();
 }
 
 }  // namespace
 
+// both sources get the same staging limit: launch_encode clamps every tile to it
 cudaError_t configure_gelf_encode(int max_tile_bytes) {
-    cudaError_t e = cudaFuncSetAttribute(gelf_size_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_tile_bytes);
+    cudaError_t e = configure_src<From5424>(max_tile_bytes);
     if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(gelf_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_tile_bytes);
+    return configure_src<From3164>(max_tile_bytes);
 }
 
 size_t gelf_scan_temp_bytes(int n) {
@@ -603,15 +667,13 @@ size_t gelf_scan_temp_bytes(int n) {
     return bytes;
 }
 
-cudaError_t launch_gelf_encode(const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream) {
+cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream) {
     if (p.n <= 0) return cudaSuccess;
-    const int grid = (p.n + kEncLines - 1) / kEncLines;
-    gelf_size_kernel<<<grid, kEncLines, p.tile_bytes, stream>>>(p);
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(d_scan_temp, scan_temp_bytes, p.lens, p.rel, p.n, stream);
-    if (e != cudaSuccess) return e;
-    gelf_base_kernel<<<1, 1, 0, stream>>>(p);
-    gelf_write_kernel<<<grid, kEncLines, p.tile_bytes, stream>>>(p);
-    return cudaGetLastError();
+    switch (fmt) {
+        case 0: return launch_src<From5424>(p, d_scan_temp, scan_temp_bytes, stream);
+        case 3: return launch_src<From3164>(p, d_scan_temp, scan_temp_bytes, stream);
+        default: return cudaErrorInvalidValue;
+    }
 }
 
 }  // namespace fg

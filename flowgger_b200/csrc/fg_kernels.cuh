@@ -138,7 +138,7 @@ cudaError_t launch_parse5424(const Parse5424Params& p, cudaStream_t stream, cuda
 cudaError_t configure_parse5424(int max_tile_bytes);
 int parse5424_smem_bytes(int tile_bytes);
 
-// ---- fused GELF encoder over the RFC5424 results (fg_gelf_encode.cu) ---------------------------------------------------
+// ---- fused GELF encoder over the RFC5424 or RFC3164 results (fg_gelf_encode.cu) ---------------------------------------
 struct GelfEncodeParams {
     const uint8_t* bytes;
     const int32_t* offsets;  // [n+1], element 0 = first line of this launch
@@ -166,9 +166,18 @@ struct GelfEncodeParams {
     const uint32_t* bad_offsets;
     uint32_t entry_cap, wide_cap, wentry_cap;  // a table that overflowed is not read (the batch is redone after a regrow)
     int32_t tile_bytes;                        // staging tile of the two kernels (dynamic shared memory)
+    // RFC3164 source: the row columns parse3164_kernel wrote for these lines (element 0 = first line of this launch);
+    // spans are absolute in `bytes`, except a message flagged FG_FLAG_MSG_ARENA, whose offset indexes `arena`
+    const double* r3_ts;
+    const uint32_t* r3_meta;
+    const int2* r3_host;
+    const int2* r3_msg;
+    const int2* r3_full;
+    uint32_t arena_cap;
 };
 cudaError_t configure_gelf_encode(int max_tile_bytes);
-cudaError_t launch_gelf_encode(const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
+// fmt: the decoder whose results the encoder reads (0 = RFC5424, 3 = RFC3164)
+cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
 size_t gelf_scan_temp_bytes(int n);
 
 // RFC5424 (short lines, staged tile): 64-line CTAs — tile waits and barriers half as wide as with 128 lines

@@ -526,7 +526,7 @@ void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
     const uint8_t dummy = 0;
     const uint8_t* bytes = arena_.empty() ? &dummy : arena_.data();
     std::lock_guard<std::mutex> guard(gpu->mutex());  // held until every Record of the batch has been materialised
-    if (fused_ != nullptr && gpu->format() == FG_FMT_RFC5424) {
+    if (fused_ != nullptr && CudaGelfEncoder::fuses_with(gpu->format())) {
         // decode + encode on the device (line_splitter.rs:50-52 fused): only the encoded records come back
         fg_encoded_out eo;
         gpu->decode_encode_gelf(bytes, offsets_.data(), n, fused_->extra(), &eo);
@@ -590,7 +590,7 @@ bool is_invalid_utf8_status(fg_format fmt, uint32_t status) {
 }
 
 // The line and NUL splitters: raw blocks of the stream, each cut after its last delimiter, are framed, checked for UTF-8
-// and decoded on the device (fg_split_decode_framed), with a CudaGelfEncoder on an RFC5424 decoder also encoded there
+// and decoded on the device (fg_split_decode_framed), with a CudaGelfEncoder on a decoder it fuses with also encoded there
 // (fg_split_decode_encode_gelf).  Records, stderr and stdout come out in stream order, exactly as the reference's
 // splitter + decoder + encoder give them.
 class BlockSplitter {
@@ -653,7 +653,7 @@ class BlockSplitter {
     bool decode_on(CudaBatchDecoder* gpu, const uint8_t* p, int64_t n) {
         std::lock_guard<std::mutex> guard(gpu->mutex());  // held until every record of the block has been emitted
         const fg_format fmt = gpu->format();
-        if (fused_ != nullptr && fmt == FG_FMT_RFC5424) {
+        if (fused_ != nullptr && CudaGelfEncoder::fuses_with(fmt)) {
             // framing + decode + encode on the device (line_splitter.rs:17-52 fused): only the encoded records come back
             fg_encoded_out eo;
             const int32_t* lines;
@@ -1139,8 +1139,8 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
     }
 }
 
-// BatchingLineSplitter (framing 0) or BatchingNulSplitter (framing 1) with output.format = "gelf" (fused decode + encode):
-// text in, one JSON record per line out
+// BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or BatchingSyslenSplitter (framing 2, through
+// RecordBatcher) with output.format = "gelf" (fused decode + encode): text in, one JSON record per line out
 int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
                           const char* const* keys, const char* const* vals, uint8_t** out_records, int64_t* out_records_len,
                           uint8_t** out_stderr, int64_t* out_stderr_len, int framing) {
@@ -1163,7 +1163,8 @@ int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max
     std::string records;
     try {
         auto tx = [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); };
-        if (framing == 1) BatchingNulSplitter(lim).run(is, tx, dec, enc, es, os);  // input.framing = "nul"
+        if (framing == 1) BatchingNulSplitter(lim).run(is, tx, dec, enc, es, os);        // input.framing = "nul"
+        else if (framing == 2) BatchingSyslenSplitter(lim).run(is, tx, dec, enc, es, os);  // input.framing = "syslen"
         else BatchingLineSplitter(lim).run(is, tx, dec, enc, es, os);
     } catch (const std::exception&) {
         return -1;

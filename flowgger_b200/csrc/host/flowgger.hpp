@@ -179,10 +179,13 @@ class Encoder {
 };
 
 // encoder/gelf_encoder.rs:10-48: output.format = "gelf".  The encoder runs FUSED with the decoder on the GPU
-// (fg_decode_encode_gelf): BatchingLineSplitter recognises this type and never materialises Records for it.
+// (fg_decode_encode_gelf) for the input formats fuses_with() accepts: the batching splitters and RecordBatcher recognise
+// this type and never materialise Records for them.
 class CudaGelfEncoder : public Encoder {
    public:
     explicit CudaGelfEncoder(std::vector<std::pair<std::string, std::string>> extra = {}) : extra_(std::move(extra)) {}
+    // the decoders whose device-resident results the fused encoder reads (fg_decode_encode_gelf)
+    static bool fuses_with(fg_format fmt) { return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164; }
     // a lone host-side Record cannot be encoded: there is no CPU encoder behind this interface
     bool encode(Record&&, std::vector<uint8_t>&, const char** err) const override {
         if (err) *err = "GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)";
@@ -198,8 +201,8 @@ class CudaGelfEncoder : public Encoder {
 // "{err}: [{line.trim()}]" to stderr): line_splitter.rs:50, nul_splitter.rs:57, syslen_splitter.rs:65,
 // input/udp_input.rs:139, input/redis_input.rs:159, input/file/worker.rs:116.  A caller frames its records as the old
 // code did and push()es each one; the batcher accumulates up to Limits, decodes the batch on the GPU in one call and then,
-// in the original order, encodes + sends every Record or prints the identical stderr line.  With a CudaGelfEncoder and an
-// RFC5424 decoder the two stages run fused on the device (fg_decode_encode_gelf).
+// in the original order, encodes + sends every Record or prints the identical stderr line.  With a CudaGelfEncoder and a
+// decoder it fuses with (CudaGelfEncoder::fuses_with) the two stages run fused on the device (fg_decode_encode_gelf).
 class CudaGelfEncoder;
 class RecordBatcher {
    public:
@@ -233,8 +236,8 @@ class RecordBatcher {
 // Batched twin of LineSplitter::run (splitter/line_splitter.rs:10-54).  It reads raw blocks of up to Limits::max_bytes
 // (at most the context's max_batch_bytes), cuts each after its last "\n" and carries the tail into the next block.  The
 // device frames the block like BufRead::lines (strip "\n" and one "\r"), checks UTF-8 (invalid => "Invalid UTF-8 input"
-// on stderr, line skipped) and decodes it (fg_split_decode_framed); with a CudaGelfEncoder and an RFC5424 decoder it also
-// encodes (fg_split_decode_encode_gelf).  A block that frames into more lines than the context holds is decoded in two
+// on stderr, line skipped) and decodes it (fg_split_decode_framed); with a CudaGelfEncoder and a decoder it fuses with
+// (CudaGelfEncoder::fuses_with) it also encodes (fg_split_decode_encode_gelf).  A block that frames into more lines than the context holds is decoded in two
 // halves cut at a "\n" near its middle; a line longer than max_batch_bytes gets a context of its own (make_sized).
 class BatchingLineSplitter {
    public:

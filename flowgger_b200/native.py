@@ -354,7 +354,9 @@ class BatchDecoder:
         self._check(self.L.fg_set_gelf_extra(self.ctx, len(ex), keys, vals), "fg_set_gelf_extra")
 
     def decode_encode_gelf(self, data: np.ndarray, offsets: np.ndarray, copy: bool = True):
-        """decode + GelfEncoder::encode fused on the device: (JSON bytes, int64 offsets[n+1], status uint8[n], kernel ms).
+        """decode + GelfEncoder::encode fused on the device, for a decoder of FMT_RFC5424 or FMT_RFC3164 (LTSV and GELF
+        raise): (JSON bytes, int64 offsets[n+1], status uint8[n], kernel ms).  An RFC3164 record has no application_name,
+        process_id or sd_id, "level" only when the line has a <PRI>, and always a "short_message" (possibly "").
         With copy=False the arrays are views of the context's pinned buffers (valid until the next call)."""
         assert data.dtype == np.uint8 and offsets.dtype == np.int32
         out = FgEncodedOut()
@@ -370,9 +372,10 @@ class BatchDecoder:
         return buf, offs, status, out.kernel_ms
 
     def split_decode_encode_gelf(self, stream: np.ndarray, framing: int = 0, copy: bool = True):
-        """Framing (0 = "line", 1 = "nul") + UTF-8 validation + decode + GelfEncoder::encode of a raw byte stream, all on
-        the device: (JSON bytes, int64 offsets[n+1], status uint8[n], record starts int32[n+1] in `stream` with their
-        terminators, kernel ms).  A record that is not UTF-8 has status 76 ("Invalid UTF-8 input") and an empty JSON record.
+        """Framing (0 = "line", 1 = "nul") + UTF-8 validation + decode (FMT_RFC5424 or FMT_RFC3164) + GelfEncoder::encode
+        of a raw byte stream, all on the device: (JSON bytes, int64 offsets[n+1], status uint8[n], record starts
+        int32[n+1] in `stream` with their terminators, kernel ms).  A record that is not UTF-8 has status 76
+        ("Invalid UTF-8 input") and an empty JSON record.
         With copy=False the arrays are views of the context's pinned buffers (valid until the next call)."""
         assert stream.dtype == np.uint8
         out = FgEncodedOut()
@@ -552,9 +555,10 @@ def clone_decode_threads(fmt: int, lines: list[bytes], nthreads: int = 2, device
 
 def splitter_run_gelf(dec: "BatchDecoder", text: bytes, extra: dict[str, str] | None = None, max_lines: int = 1 << 16,
                       max_bytes: int = 16 << 20, framing: int = 0) -> tuple[bytes, bytes]:
-    """BatchingLineSplitter (framing 0) or BatchingNulSplitter (framing 1) with input.format = rfc5424 and
-    output.format = gelf (framing, decode and encode fused on the GPU): returns (JSON records separated by newlines,
-    stderr text)."""
+    """BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or BatchingSyslenSplitter (framing 2: records
+    framed on the host and batched by RecordBatcher) with input.format = rfc5424 or rfc3164 (the decoder's format) and
+    output.format = gelf (decode and encode fused on the GPU, framing too for 0 and 1): returns (JSON records separated
+    by newlines, stderr text)."""
     H = load_host()
     ex = list((extra or {}).items())
     keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])

@@ -250,13 +250,16 @@ int fg_flush_l2(fg_ctx* ctx); /* writes a >L2-sized scratch buffer */
 
 /* ---- decode + encode fused on the device (SURVEY.md 8(f) N2) ------------------------------------------------------
  * The reference calls Encoder::encode right after Decoder::decode for every record (splitter/line_splitter.rs:50-52).
- * For the default pair input.format = "rfc5424" / output.format = "gelf" both stages run on the GPU and only the
- * encoded records come back:
+ * For output.format = "gelf" with input.format = "rfc5424" (the default pair) or "rfc3164" both stages run on the GPU
+ * and only the encoded records come back:
  *     GelfEncoder::new(&Config)   encoder/gelf_encoder.rs:29-48   -> fg_set_gelf_extra (output.gelf_extra)
  *     Encoder::encode(Record)     encoder/gelf_encoder.rs:59-115, encoder/mod.rs:54-56 -> fg_decode_encode_gelf
  * Record i is bytes[offsets[i], offsets[i+1]) — exactly the Vec<u8> the reference's encode returns (serde_json 0.8
  * text: keys in byte order, later inserts replace earlier ones, no whitespace); a line the decoder rejects has
- * status[i] != 0 (fg_error_string) and an empty record. */
+ * status[i] != 0 (fg_error_string) and an empty record.  An RFC3164 record has no application_name, process_id or sd_id
+ * (the Record holds None for them; a gelf_extra of that key is still written), "level" only when the line has a <PRI>,
+ * and "short_message" always (possibly ""), as rfc3164_decoder.rs builds it.  The year of a timestamp without one is
+ * fixed at the start of each call (fg_set_rfc3164_year).  LTSV and GELF input -> FG_E_ARG. */
 typedef struct fg_encoded_out {
     int32_t n;
     const uint8_t* bytes;     /* concatenated records */
@@ -266,16 +269,16 @@ typedef struct fg_encoded_out {
     float total_ms;
 } fg_encoded_out;
 int fg_set_gelf_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
-int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 */, const uint8_t* bytes, const int32_t* offsets, int32_t n,
-                          fg_encoded_out* out);
-/* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424 decode ->
- * GelfEncoder::encode, all on the device; only the encoded records and the record extents come back.
+int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 */, const uint8_t* bytes, const int32_t* offsets,
+                          int32_t n, fg_encoded_out* out);
+/* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424 or RFC3164
+ * decode -> GelfEncoder::encode, all on the device; only the encoded records and the record extents come back.
  * Record i is out->bytes[out->offsets[i], out->offsets[i+1]); out->status[i] is 0, a decoder status, or the framing status
  * whose fg_error_string is "Invalid UTF-8 input" (empty record).  *line_offsets ([n+1], starts in `stream`, each record
  * still carrying its terminator, like fg_batch_out.line_offsets) stays valid until the next call on the context.
- * Errors: another format or an unknown framing -> FG_E_ARG; nbytes > max_batch_bytes or more records than
+ * Errors: LTSV or GELF input or an unknown framing -> FG_E_ARG; nbytes > max_batch_bytes or more records than
  * max_batch_lines -> FG_E_CAPACITY (the context stays usable). */
-int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 */, fg_framing framing, const uint8_t* stream,
+int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 */, fg_framing framing, const uint8_t* stream,
                                 int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
 
 /* the reference's Err(&'static str) for a row status (0 -> NULL) */

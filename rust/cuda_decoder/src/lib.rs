@@ -7,7 +7,7 @@
 //!   * `Splitter<T>::run`                                                    (src/flowgger/splitter/mod.rs:18-26)
 //! All parsing happens on the GPU — including line framing, the UTF-8 check and the unescape of RFC5424 SD values; this
 //! crate hands raw blocks to `fg_split_decode` (or packed lines to `fg_decode_batch`) and materialises Records, or, for
-//! the rfc5424 -> gelf pair, forwards the records the device already framed, decoded and encoded
+//! the rfc5424 -> gelf and rfc3164 -> gelf pairs, forwards the records the device already framed, decoded and encoded
 //! (`fg_split_decode_encode_gelf`).
 #![allow(non_camel_case_types, non_upper_case_globals, dead_code)]
 
@@ -216,7 +216,8 @@ impl CudaDecoder {
     }
 
     /// Framing + UTF-8 validation + decode + `GelfEncoder::encode` of a raw stream on the device
-    /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424"): `f(line, Ok(json) | Err(error))` in stream order, `line`
+    /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424" or "rfc3164", see `fuses_with_gelf`): `f(line, Ok(json) |
+    /// Err(error))` in stream order, `line`
     /// without its terminator.  false (nothing decoded) when the stream does not fit the context.
     pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>)>(&self, stream: &[u8], extra: &[(String, String)],
                                                                                    mut f: F) -> bool {
@@ -560,9 +561,16 @@ impl<T: Read> Splitter<T> for BatchingLineSplitter {
     }
 }
 
-/// `output.format = "gelf"` with `input.format = "rfc5424"`: framing, the UTF-8 check, decode AND encode run on the device
-/// (`fg_split_decode_encode_gelf`, replaces BufRead::lines + Decoder::decode + GelfEncoder::encode of
-/// line_splitter.rs:17-52); it reads raw blocks like `BatchingLineSplitter` and only the encoded records come back.
+/// The `input.format` values whose decoder runs fused with the GELF encoder on the device (`fg_decode_encode_gelf`,
+/// `fg_split_decode_encode_gelf`); `FusedGelfLineSplitter` takes a `CudaDecoder` of one of them.
+pub fn fuses_with_gelf(input_format: &str) -> bool {
+    matches!(input_format, "rfc5424" | "rfc3164")
+}
+
+/// `output.format = "gelf"` with `input.format = "rfc5424"` or `"rfc3164"` (`fuses_with_gelf`): framing, the UTF-8 check,
+/// decode AND encode run on the device (`fg_split_decode_encode_gelf`, replaces BufRead::lines + Decoder::decode +
+/// GelfEncoder::encode of line_splitter.rs:17-52); it reads raw blocks like `BatchingLineSplitter` and only the encoded
+/// records come back.  An RFC3164 context fixes the year of year-less timestamps at the start of each call.
 pub struct FusedGelfLineSplitter {
     pub gpu: CudaDecoder,
     pub extra: Vec<(String, String)>,   // output.gelf_extra (gelf_encoder.rs:29-48)

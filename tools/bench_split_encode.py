@@ -1,10 +1,14 @@
-"""Framing on the device vs on the host for the default pipeline (input.format = "rfc5424", output.format = "gelf").
+"""Framing on the device vs on the host for the fused GELF pipelines (output.format = "gelf", input.format = "rfc5424",
+the default pair, or "rfc3164").
 
-    python tools/bench_split_encode.py [--lines 10000000] [--steps 10] [--warmup 2] [--splitter-gb 1.0] [--splitter-only]
+    python tools/bench_split_encode.py [--format rfc5424|rfc3164] [--lines 10000000] [--steps 10] [--warmup 2]
+                                       [--splitter-gb 1.0] [--splitter-only]
 
-On the C2 RFC5424 workload of bench.py (seed 5424, the same mean line length), joined with '\\n' in pinned memory:
-  1. fg_split_decode_encode_gelf on the raw stream and fg_decode_encode_gelf on the same lines framed beforehand, timed
-     alternately after warm-ups; both must return byte-identical records and statuses;
+On the workload of bench.py for the format (rfc5424: C2, seed 5424; rfc3164: seed 3164, year 2026; the same mean line
+length), joined with '\\n' in pinned memory:
+  1. fg_split_decode_encode_gelf on the raw stream and fg_decode_encode_gelf on the same lines framed beforehand (for
+     rfc3164 also fg_split_decode on the raw stream: decode only, rows + arena back), timed alternately after warm-ups;
+     the two encoding calls must return byte-identical records and statuses;
   2. the C++ BatchingLineSplitter with the fused GELF encoder end to end over at least --splitter-gb of the same text
      (text in, every JSON record handed to the sender, stderr captured).
 Prints one JSON line per section, with the card's name and power limit.  --splitter-only runs section 2 alone."""
@@ -24,7 +28,9 @@ sys.path.insert(0, str(REPO))
 
 import flowgger_b200 as fb  # noqa: E402
 
-SEED, MEAN = 5424, 169.2  # bench.py: SEEDS["rfc5424"], GEN_MEAN["rfc5424"]
+# bench.py: SEEDS, GEN_MEAN and RFC3164_YEAR (the year of a timestamp without one, fixed so that a run is reproducible)
+WORKLOADS = {"rfc5424": (fb.FMT_RFC5424, 5424, 169.2), "rfc3164": (fb.FMT_RFC3164, 3164, 140.0)}
+RFC3164_YEAR = 2026
 
 
 def card() -> dict:
@@ -37,9 +43,15 @@ def card() -> dict:
         return {"gpu": None, "error": str(e)}
 
 
-def workload(n: int) -> tuple[np.ndarray, np.ndarray]:
+def workload(fmt_name: str, n: int) -> tuple[np.ndarray, np.ndarray]:
     """the raw stream (every line followed by '\\n') and its line offsets, terminators included"""
-    return fb.generate(fb.FMT_RFC5424, SEED, n, mean_len=MEAN, bad_frac=0.005, nthreads=32, terminated=True)
+    fmt, seed, mean = WORKLOADS[fmt_name]
+    return fb.generate(fmt, seed, n, mean_len=mean, bad_frac=0.005, nthreads=32, terminated=True)
+
+
+def decoder(fmt_name: str, **kw) -> fb.BatchDecoder:
+    fmt = WORKLOADS[fmt_name][0]
+    return fb.BatchDecoder(fmt, rfc3164_year=RFC3164_YEAR if fmt == fb.FMT_RFC3164 else 0, **kw)
 
 
 def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> None:
@@ -48,8 +60,9 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
     lines = stream[keep]
     loffs = (soffs - np.arange(n + 1, dtype=np.int64)).astype(np.int32)
     del keep
-    split = fb.BatchDecoder(fb.FMT_RFC5424, max_batch_bytes=len(stream) + (1 << 20), max_batch_lines=n + 64)
-    pre = fb.BatchDecoder(fb.FMT_RFC5424, max_batch_bytes=len(stream) + (1 << 20), max_batch_lines=n + 64)
+    cap = dict(max_batch_bytes=len(stream) + (1 << 20), max_batch_lines=n + 64)
+    split, pre = decoder(args.format, **cap), decoder(args.format, **cap)
+    decode = decoder(args.format, **cap) if args.format == "rfc3164" else None
     try:
         hs = split.host_alloc(len(stream))
         hs[:] = stream
@@ -58,11 +71,17 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
         ho = pre.host_alloc(loffs.nbytes, dtype=np.int32)
         ho[:] = loffs
         del lines
+        hd = None
+        if decode is not None:
+            hd = decode.host_alloc(len(stream))
+            hd[:] = stream
         for _ in range(args.warmup):
             split.split_decode_encode_gelf(hs, copy=False)
             pre.decode_encode_gelf(hl, ho, copy=False)
-        t = {"split": [], "pre": []}
-        k = {"split": [], "pre": []}
+            if decode is not None:
+                decode.split_decode(hd)
+        t = {"split": [], "pre": [], "decode": []}
+        k = {"split": [], "pre": [], "decode": []}
         framing_ms = []
         for _ in range(args.steps):
             t0 = time.perf_counter()
@@ -74,15 +93,22 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
             _, _, _, km = pre.decode_encode_gelf(hl, ho, copy=False)
             t["pre"].append(time.perf_counter() - t0)
             k["pre"].append(km)
+            if decode is not None:
+                t0 = time.perf_counter()
+                res = decode.split_decode(hd)
+                t["decode"].append(time.perf_counter() - t0)
+                k["decode"].append(res.kernel_ms)
         sb, so, ss, sl, _ = split.split_decode_encode_gelf(hs, copy=False)
         pb, po, ps, _ = pre.decode_encode_gelf(hl, ho, copy=False)
         assert len(ss) == n and np.array_equal(sl, soffs), "the device framed other lines than the generator made"
         assert np.array_equal(so, po) and np.array_equal(ss, ps) and np.array_equal(sb, pb), \
             "fg_split_decode_encode_gelf and fg_decode_encode_gelf disagree"
         out_bytes = int(so[-1])
-        for key, api, in_bytes in (("split", "fg_split_decode_encode_gelf (pinned raw stream in)", len(stream)),
-                                   ("pre", "fg_decode_encode_gelf (pinned lines + int32 offsets in, framed beforehand)",
-                                    int(loffs[-1]) + loffs.nbytes)):
+        sections = [("split", "fg_split_decode_encode_gelf (pinned raw stream in)", len(stream)),
+                    ("pre", "fg_decode_encode_gelf (pinned lines + int32 offsets in, framed beforehand)", int(loffs[-1]) + loffs.nbytes)]
+        if decode is not None:
+            sections.append(("decode", "fg_split_decode (pinned raw stream in, decode only: rows + arena back, no JSON)", len(stream)))
+        for key, api, in_bytes in sections:
             med = float(np.median(t[key]))
             rec = {"section": key, "api": api, "lines": n, "input_bytes": in_bytes, "json_bytes": out_bytes,
                    "records": int((ss == 0).sum()), "steps": args.steps, "call_ms_median": med * 1e3,
@@ -91,10 +117,15 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
                    "kernel_ms_median": float(np.median(k[key])), **info}
             if key == "split":
                 rec["framing_stage_ms_median"] = float(np.median(framing_ms))
+            if key == "decode":
+                for x in ("json_bytes", "output_gb_per_s"):
+                    del rec[x]
             print(json.dumps(rec), flush=True)
     finally:
         split.close()
         pre.close()
+        if decode is not None:
+            decode.close()
 
 
 def splitter(args, stream: np.ndarray, info: dict) -> None:
@@ -107,7 +138,7 @@ def splitter(args, stream: np.ndarray, info: dict) -> None:
         cuts.append(cuts[-1] + int(np.flatnonzero(stream[cuts[-1]:end] == ord("\n"))[-1]) + 1 if end < len(stream) else end)
     texts = [stream[a:b].tobytes() for a, b in zip(cuts[:-1], cuts[1:])]
     want = int(args.splitter_gb * 1e9)
-    dec = fb.BatchDecoder(fb.FMT_RFC5424, max_batch_bytes=64 << 20, max_batch_lines=1 << 20)
+    dec = decoder(args.format, max_batch_bytes=64 << 20, max_batch_lines=1 << 20)
     wall, in_bytes, json_bytes, lines, n_rec, n_err = 0.0, 0, 0, 0, 0, 0
     try:
         small = texts[0][: 1 << 20]
@@ -135,6 +166,7 @@ def splitter(args, stream: np.ndarray, info: dict) -> None:
 
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--format", choices=sorted(WORKLOADS), default="rfc5424")
     ap.add_argument("--lines", type=int, default=10_000_000)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
@@ -142,7 +174,9 @@ def main() -> None:
     ap.add_argument("--splitter-only", action="store_true")
     args = ap.parse_args()
     info = card()
-    stream, soffs = workload(args.lines)
+    if args.format != "rfc5424":
+        info["format"] = args.format
+    stream, soffs = workload(args.format, args.lines)
     if not args.splitter_only:
         device_paths(args, stream, soffs, info)
     splitter(args, stream, info)
