@@ -218,7 +218,7 @@ struct fg_ctx {
     Buf<fg::Row5424, fg_row5424> rows5;
     Buf<uint32_t> esc_list, wide_list;
     // fused GELF encoder (fg_decode_encode_gelf)
-    Buf<uint32_t> enc_lens, enc_rel;
+    Buf<unsigned long long> enc_lens, enc_rel;  // record lengths and their sum inside a launch: a launch may pass 4 GiB
     Buf<unsigned long long> enc_base;  // [chunks + 1] running output size
     Buf<uint8_t> enc_out;
     size_t enc_out_cap = 0;  // enc_out holds 16 bytes more

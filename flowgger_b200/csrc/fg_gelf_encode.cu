@@ -41,9 +41,10 @@ struct Span {
     int len;
 };
 
+// record lengths are 64-bit all the way to the output offsets: one record, or one launch's records, may pass 4 GiB
 struct CountSink {
-    uint32_t n = 0;
-    __device__ __forceinline__ void push(uint32_t, int k) { n += (uint32_t)k; }
+    unsigned long long n = 0;
+    __device__ __forceinline__ void push(uint32_t, int k) { n += (unsigned)k; }
     __device__ __forceinline__ void finish() {}
 };
 // bytes -> aligned 32-bit stores: a 64-bit shift register takes 1 or 4 bytes per push (the same instructions for both, so
@@ -597,14 +598,14 @@ __global__ void __launch_bounds__(kEncLines) gelf_size_kernel(const __grid_const
     CountSink s;
     emit_record<Src>(P, B, r, r.ok, s);
     if (!valid) return;
-    P.lens[i] = r.ok ? s.n : 0u;
+    P.lens[i] = r.ok ? s.n : 0ull;
     P.status[i] = (uint8_t)Src::status(P, i);
 }
 
 // chunk totals: base[k + 1] = base[k] + bytes of this chunk (one thread)
 __global__ void gelf_base_kernel(const __grid_constant__ GelfEncodeParams P) {
     if (*P.bad_offsets) return;
-    const unsigned long long total = (unsigned long long)P.rel[P.n - 1] + P.lens[P.n - 1];
+    const unsigned long long total = P.rel[P.n - 1] + P.lens[P.n - 1];
     P.base[1] = P.base[0] + total;
 }
 
@@ -617,8 +618,7 @@ __global__ void __launch_bounds__(kEncLines) gelf_write_kernel(const __grid_cons
     const ByteSource B = stage_lines(P, tile, &sh.mbar, first, last);
     const int i = sorted_line(P, sh, first, last);
     const bool valid = i >= 0;
-    unsigned long long at = 0;
-    uint32_t len = 0;
+    unsigned long long at = 0, len = 0;
     if (valid) {
         at = P.base[0] + P.rel[i];
         len = P.lens[i];
@@ -626,7 +626,7 @@ __global__ void __launch_bounds__(kEncLines) gelf_write_kernel(const __grid_cons
         if (i == P.n - 1) P.out_offsets[P.n] = (long long)(at + len);
     }
     // a rejected line has no record; an output buffer that overflowed is not written (the batch is redone)
-    const bool live = valid && len != 0u && at + len <= P.out_cap;
+    const bool live = valid && len != 0ull && at + len <= P.out_cap;
     RecView r;
     r.ok = false;
     if (live) Src::load(P, B, i, r);
@@ -663,7 +663,7 @@ cudaError_t configure_gelf_encode(int max_tile_bytes) {
 
 size_t gelf_scan_temp_bytes(int n) {
     size_t bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, n);
+    cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const unsigned long long*)nullptr, (unsigned long long*)nullptr, n);
     return bytes;
 }
 

@@ -156,8 +156,8 @@ struct GelfEncodeParams {
     const int32_t* static_key_off;  // [n_static+1] raw key bytes (for ordering against the SD names)
     const int32_t* static_lit_off;  // [n_static+1] text to emit: `"key":`, for an extra `"key":"value"`
     const int32_t* static_kind;     // [n_static] GF_*
-    uint32_t* lens;                 // [n] record lengths (size pass)
-    uint32_t* rel;                  // [n] exclusive sum of lens inside this launch
+    unsigned long long* lens;       // [n] record lengths (size pass)
+    unsigned long long* rel;        // [n] exclusive sum of lens inside this launch
     unsigned long long* base;       // base[0] = output bytes before this launch, base[1] receives base[0] + this launch's bytes
     uint8_t* out;
     unsigned long long out_cap;
