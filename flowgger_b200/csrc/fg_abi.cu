@@ -192,6 +192,7 @@ struct fg_ctx {
     size_t max_bytes = 0;
     int max_lines = 0;
     int chunk_lines = 0;
+    int input_format = 0;  // fg_config.input_format
     Stream s_h2d, s_comp, s_d2h;
     Stream s_parse;  // split mode: the parse kernels, behind the framing on s_comp
     Event ev_a, ev_b;
@@ -224,6 +225,8 @@ struct fg_ctx {
     size_t enc_out_cap = 0;  // enc_out holds 16 bytes more
     Buf<long long, int64_t> enc_offsets;
     Buf<uint8_t> enc_status;
+    Buf<int32_t> enc_stop;  // LTSV: where the decoder stopped printing "Missing value" lines (fg_encoded_ltsv_stops)
+    int enc_stop_n = -1;    // records of the last fused LTSV call (-1: the last fused call was not LTSV)
     Buf<uint8_t> scan_temp;
     size_t scan_temp_bytes = 0;
     Buf<uint8_t> static_blob;  // fixed GELF keys + output.gelf_extra, sorted
@@ -566,8 +569,11 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
     return FG_OK;
 }
 
-// The decoders whose device-resident results the fused GELF encoder reads
-bool gelf_fusable(int fmt) { return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164; }
+// The decoders whose device-resident results the fused GELF encoder reads.  LTSV only on a context created for it: the
+// pair keys carry that context's ltsv_suffixes.
+bool gelf_fusable(const fg_ctx* c, int fmt) {
+    return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || (fmt == FG_FMT_LTSV && c->input_format == FG_FMT_LTSV);
+}
 
 // The fused GELF encoder over the decoder's results of lines [l0, l0 + n), parse step k
 int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream_t s) {
@@ -579,11 +585,17 @@ int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream
         E.rows = reinterpret_cast<const uint4*>(c->rows5.d + l0);
     } else {
         const uint8_t* r = c->rows.d;
-        E.r3_ts = (const double*)(r + col_off(c, C_TS)) + l0;
-        E.r3_meta = (const uint32_t*)(r + col_off(c, C_META)) + l0;
-        E.r3_host = (const int2*)(r + col_off(c, C_HOST)) + l0;
-        E.r3_msg = (const int2*)(r + col_off(c, C_MSG)) + l0;
-        E.r3_full = (const int2*)(r + col_off(c, C_FULL)) + l0;
+        E.col_ts = (const double*)(r + col_off(c, C_TS)) + l0;
+        E.col_meta = (const uint32_t*)(r + col_off(c, C_META)) + l0;
+        E.col_host = (const int2*)(r + col_off(c, C_HOST)) + l0;
+        E.col_msg = (const int2*)(r + col_off(c, C_MSG)) + l0;
+        E.col_full = (const int2*)(r + col_off(c, C_FULL)) + l0;
+    }
+    if (fmt == FG_FMT_LTSV) {
+        E.col_sd = (const int2*)(c->rows.d + col_off(c, C_SD)) + l0;
+        E.ltsv_suffix = c->ltsv.suffix;
+        for (int t = 0; t < 6; ++t) E.ltsv_suffix_off[t] = c->ltsv.suffix_off[t];
+        E.ltsv_stop = c->enc_stop.d + l0;
     }
     E.entries = dev<unsigned long long>(c, T_E8);
     E.arena = dev<uint8_t>(c, T_ARENA);
@@ -780,6 +792,8 @@ int parse_step(fg_ctx* c, int fmt, int k, int l0, int n, int tile, const uint8_t
     if (!encode) return copy_rows_d2h(c, fmt, l0, n, c->s_d2h);
     FG_CUDA(c, cudaMemcpyAsync(c->enc_status.h + l0, c->enc_status.d + l0, (size_t)n, cudaMemcpyDeviceToHost, c->s_d2h));
     FG_CUDA(c, cudaMemcpyAsync(c->enc_offsets.h + l0, c->enc_offsets.d + l0, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, c->s_d2h));
+    if (fmt == FG_FMT_LTSV)
+        FG_CUDA(c, cudaMemcpyAsync(c->enc_stop.h + l0, c->enc_stop.d + l0, (size_t)n * 4, cudaMemcpyDeviceToHost, c->s_d2h));
     return FG_OK;
 }
 
@@ -954,8 +968,9 @@ int grow_enc_out(fg_ctx* c, size_t cap) {
     return FG_OK;
 }
 
-int ensure_encoder(fg_ctx* c, int chunks) {
+int ensure_encoder(fg_ctx* c, int fmt, int chunks) {
     const size_t L = (size_t)c->max_lines;
+    if (fmt == FG_FMT_LTSV && !c->enc_stop.d) FG_CUDA(c, c->enc_stop.alloc(L, BOTH));
     if (!c->enc_lens.d) {
         FG_CUDA(c, c->enc_lens.alloc(L, DEV));
         FG_CUDA(c, c->enc_rel.alloc(L, DEV));
@@ -1025,6 +1040,7 @@ int fg_create(const fg_config* cfg, fg_ctx** out) {
     c->chunk_lines = cfg->chunk_lines > 0 ? cfg->chunk_lines : (512 << 10);
     c->chunk_lines = (c->chunk_lines + 127) / 128 * 128;  // a multiple of every kernel's lines per CTA
     c->r3164_year = cfg->rfc3164_year;
+    c->input_format = cfg->input_format;
     if (cfg->tzdir) c->tzdir = cfg->tzdir;
     if (int rc = init_device(c, cfg)) {
         fprintf(stderr, "flowgger_cuda: %s\n", c->last_error.c_str());
@@ -1176,22 +1192,25 @@ int fg_set_gelf_extra(fg_ctx* c, int32_t n, const char* const* keys, const char*
     return build_static_items(c);
 }
 
-// decode (RFC5424 or RFC3164) + GelfEncoder::encode fused: H2D lines -> parse kernels -> size / scan / write kernels ->
-// D2H of the encoded records only, chunk by chunk; the decoder's rows and side tables never leave the device.
+// decode (RFC5424, RFC3164 or LTSV) + GelfEncoder::encode fused: H2D lines -> parse kernels -> size / scan / write
+// kernels -> D2H of the encoded records (and for LTSV the "Missing value" stops) only, chunk by chunk; the decoder's rows
+// and side tables never leave the device.
 int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
     if (!c || !out) return FG_E_ARG;
+    c->enc_stop_n = -1;  // the stops of an earlier call end here, whatever this one returns
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
-    if (!gelf_fusable((int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
+    if (!gelf_fusable(c, (int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
     if (int rc = begin_call(c, fmt)) return rc;
     const int C = c->chunk_lines;
     const int chunks = n > 0 ? (n + C - 1) / C : 1;
-    if (int rc = ensure_encoder(c, chunks)) return rc;
+    if (int rc = ensure_encoder(c, (int)fmt, chunks)) return rc;
     memset(out, 0, sizeof *out);
     out->bytes = c->enc_out.h;
     out->offsets = c->enc_offsets.h;
     out->status = c->enc_status.h;
     if (n == 0) {
         c->enc_offsets.h[0] = 0;
+        if (fmt == FG_FMT_LTSV) c->enc_stop_n = 0;
         return FG_OK;
     }
     const auto t_begin = std::chrono::steady_clock::now();
@@ -1223,9 +1242,16 @@ int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const 
         out->n = n;
         out->kernel_ms = kms;
         out->total_ms = tms;
+        if (fmt == FG_FMT_LTSV) c->enc_stop_n = n;
         return FG_OK;
     }
     return fail(c, FG_E_CAPACITY, "output / side table overflow after regrow");
+}
+
+int fg_encoded_ltsv_stops(const fg_ctx* c, const int32_t** stop) {
+    if (!c || !stop || c->enc_stop_n < 0) return FG_E_ARG;
+    *stop = c->enc_stop.h;
+    return FG_OK;
 }
 
 }  // extern "C"
@@ -1248,7 +1274,7 @@ int split_stream(fg_ctx* c, int fmt, fg_framing framing, const uint8_t* stream, 
     constexpr long long kChunk = 64ll << 20;  // pipeline granularity in bytes (a multiple of the 8 KB framing segment)
     const int chunks = nbytes > 0 ? (int)((nbytes + kChunk - 1) / kChunk) : 1;
     if (encode)
-        if (int rc = ensure_encoder(c, chunks)) return rc;  // at most one parse step per chunk
+        if (int rc = ensure_encoder(c, fmt, chunks)) return rc;  // at most one parse step per chunk
     if (!c->seg.d) {
         FG_CUDA(c, c->seg.alloc((size_t)fg::split_segments((long long)c->max_bytes) + 16, DEV));
         FG_CUDA(c, c->n_lines.alloc(64, BOTH));
@@ -1372,16 +1398,18 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
     return FG_OK;
 }
 
-// framing + decode (RFC5424 or RFC3164) + GelfEncoder::encode on the device: only the encoded records and the line
-// offsets come back
+// framing + decode (RFC5424, RFC3164 or LTSV) + GelfEncoder::encode on the device: only the encoded records, the line
+// offsets and for LTSV the "Missing value" stops come back
 int fg_split_decode_encode_gelf(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
                                 const int32_t** line_offsets) {
     if (!c || !out || !line_offsets) return FG_E_ARG;
-    if (!gelf_fusable((int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
+    c->enc_stop_n = -1;  // the stops of an earlier call end here, whatever this one returns
+    if (!gelf_fusable(c, (int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
     int32_t n;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;
     if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, true, n, total, kms, tms)) return rc;
+    if (fmt == FG_FMT_LTSV) c->enc_stop_n = n;
     memset(out, 0, sizeof *out);
     out->n = n;
     out->bytes = c->enc_out.h;

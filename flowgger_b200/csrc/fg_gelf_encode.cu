@@ -6,11 +6,15 @@
 // an earlier one (SD pairs replace fixed fields, output.gelf_extra replaces everything), compact separators, strings
 // with `"` `\\` \b \f \n \r \t escaped, Record.ts through dtoa (fg_dtoa.cuh).
 //
-// Input = the decoder's device-resident results; nothing of them travels to the host in this mode.  Two record sources,
-// chosen at compile time (the kernels are templates on the source, everything after the record view is shared):
+// Input = the decoder's device-resident results; nothing of them travels to the host in this mode.  Three record
+// sources, chosen at compile time (the kernels are templates on the source, everything after the record view is shared):
 //   From5424  compact rows + 8-byte entries + arena, or wide rows (structured data; every fixed field present)
 //   From3164  the row columns of parse3164_kernel + the arena of re-joined messages (rfc3164_decoder.rs:71-82, 106-117:
 //             no appname, procid or structured data; no severity without <PRI>; msg always Some, possibly "")
+//   FromLtsv  the row columns of parse_ltsv_kernel + its 17-byte side table (ltsv_decoder.rs:87-221: no appname, procid
+//             or sd_id; no severity without `level`; msg None without `message`).  A pair's key is '_' + name + the
+//             type's suffix (FG_EM_SUFFIX), so keys are ordered and de-duplicated on that composed text; a typed value
+//             (bool, f64, i64, u64) is written as JSON, not as its source text.
 // Launches per chunk of lines:
 //   gelf_size_kernel   one thread per line: exact length of its record (0 for a line the decoder rejected); the bytes of
 //                      the CTA's 256 lines are staged in shared memory by one TMA bulk copy and handed to the threads
@@ -80,6 +84,15 @@ struct WordSink {
         for (int k = 0; k < nacc; ++k) p[k] = (uint8_t)(acc >> (8 * k));
         nacc = 0;
     }
+};
+
+// An LTSV record's sink: the extent of the side table's value column, which tells run_segments the number segments
+template <class Sink>
+struct NumSink {
+    Sink& s;
+    const unsigned long long* vals;
+    uint32_t cap;
+    __device__ __forceinline__ void push(uint32_t w, int k) { s.push(w, k); }
 };
 
 // byte-order comparison of ('_' + a) with b
@@ -180,15 +193,15 @@ constexpr uint32_t kNoSeverity = 0xFFu;  // a line without <PRI>: Record.severit
 
 // An RFC3164 row: absolute spans (fg_parse3164.cu).  msg is never None: an empty message still gets a non-null pointer.
 __device__ __forceinline__ void load_view_3164(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) {
-    const uint32_t meta = P.r3_meta[i];
+    const uint32_t meta = P.col_meta[i];
     r.ok = (meta & 0xFFu) == 0u;
     r.wide = false;
     r.has_sd = false;
     r.first = r.count = 0;
     if (!r.ok) return;
     r.severity = (meta >> 16) & 0xFFu;
-    r.ts = P.r3_ts[i];
-    const int2 h = P.r3_host[i], m = P.r3_msg[i], f = P.r3_full[i];
+    r.ts = P.col_ts[i];
+    const int2 h = P.col_host[i], m = P.col_msg[i], f = P.col_full[i];
     r.host = Span{B.at(h.x), h.y};
     r.full = Span{B.at(f.x), f.y};
     if ((meta >> 24) & kMsgArena) {
@@ -199,18 +212,25 @@ __device__ __forceinline__ void load_view_3164(const GelfEncodeParams& P, const 
     }
 }
 
-// The record sources the kernels are instantiated for.  kSd: the record may carry structured data.  kOptional:
-// application_name and process_id are None, and level is None without a severity.
-struct From5424 {
-    static constexpr bool kSd = true, kOptional = false;
-    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view(P, B, i, r); }
-    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.rows[2 * (size_t)i].z & 0xFFu; }
-};
-struct From3164 {
-    static constexpr bool kSd = false, kOptional = true;
-    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_3164(P, B, i, r); }
-    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.r3_meta[i] & 0xFFu; }
-};
+// An LTSV row: the column layout of RFC3164 (absolute spans, fg_parse_ltsv.cu) plus sd = its rows of the side table.
+// msg.x < 0: the line has no `message` part (None, written "-"); `message:` is Some("") and gets a non-null pointer.
+__device__ __forceinline__ void load_view_ltsv(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) {
+    const uint32_t meta = P.col_meta[i];
+    r.ok = (meta & 0xFFu) == 0u;
+    r.wide = false;
+    r.has_sd = false;
+    r.first = r.count = 0;
+    if (!r.ok) return;
+    r.severity = (meta >> 16) & 0xFFu;
+    r.ts = P.col_ts[i];
+    const int2 h = P.col_host[i], m = P.col_msg[i], f = P.col_full[i], sd = P.col_sd[i];
+    r.host = Span{B.at(h.x), h.y};
+    r.full = Span{B.at(f.x), f.y};
+    r.msg = m.x >= 0 ? Span{B.at(m.x), m.y} : Span{nullptr, 0};
+    r.first = (uint32_t)sd.x;
+    r.count = (uint32_t)sd.y;
+    if ((unsigned long long)r.first + r.count > (unsigned long long)P.wentry_cap) r.ok = false;
+}
 
 // pair e of the line (false: the row is an element header)
 __device__ __forceinline__ bool load_pair(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, uint32_t e, Span& name,
@@ -234,6 +254,109 @@ __device__ __forceinline__ bool load_pair(const GelfEncodeParams& P, const ByteS
         val = Span{r.line + ne + 2, (int)((v >> 32) & 0xFFFFu) - (ne + 2)};
     }
     return true;
+}
+
+// An LTSV pair.  Its key after the '_' is name + suffix (ltsv_decoder.rs:131-193: the type's suffix when the entry has
+// FG_EM_SUFFIX), so two different names can give the same key; tag 0: a string value (v = offset | length << 32), else
+// the fg_ltsv_type of the 8 value bytes in v.
+struct LtsvKey {
+    Span name, suffix;
+};
+struct LtsvVal {
+    unsigned long long v;
+    uint32_t tag;
+    uint32_t e;  // its row
+};
+constexpr uint32_t kEmSuffix = 0x20u;  // FG_EM_SUFFIX
+
+__device__ __forceinline__ bool load_pair_ltsv(const GelfEncodeParams& P, const ByteSource& B, uint32_t e, LtsvKey& key, LtsvVal& val) {
+    const uint32_t m = P.wentry_meta[e], t = m & 0x07u;
+    const int2 nm = P.wentry_name[e];
+    key.name = Span{B.at(nm.x), nm.y};
+    key.suffix = Span{nullptr, 0};
+    if (m & kEmSuffix) {
+        const int a = P.ltsv_suffix_off[t];
+        key.suffix = Span{P.ltsv_suffix + a, P.ltsv_suffix_off[t + 1] - a};
+    }
+    val.v = P.wentry_val[e];
+    val.tag = t;
+    val.e = e;
+    return true;
+}
+
+// byte k of the composed key (after the '_')
+__device__ __forceinline__ uint32_t key_byte(const LtsvKey& a, int k) {
+    return k < a.name.len ? a.name.p[k] : a.suffix.p[k - a.name.len];
+}
+__device__ __forceinline__ int key_len(const LtsvKey& a) { return a.name.len + a.suffix.len; }
+__device__ __forceinline__ uint32_t name_prefix(const LtsvKey& n) {
+    uint32_t k = 0;
+    for (int j = 0; j < 4; ++j) k = (k << 8) | (j < key_len(n) ? key_byte(n, j) : 0u);
+    return k;
+}
+__device__ __forceinline__ int cmp_names(const LtsvKey& a, const LtsvKey& b) {
+    const int la = key_len(a), lb = key_len(b), n = min(la, lb);
+    for (int k = 0; k < n; ++k) {
+        const uint32_t x = key_byte(a, k), y = key_byte(b, k);
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return la == lb ? 0 : (la < lb ? -1 : 1);
+}
+// byte-order comparison of ('_' + name + suffix) with b
+__device__ __forceinline__ int cmp_sd_key(const LtsvKey& a, Span b) {
+    if (b.len == 0) return 1;
+    if ((uint32_t)'_' != b.p[0]) return (uint32_t)'_' < b.p[0] ? -1 : 1;
+    const int la = key_len(a), n = min(la, b.len - 1);
+    for (int k = 0; k < n; ++k) {
+        const uint32_t x = key_byte(a, k), y = b.p[k + 1];
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return la == b.len - 1 ? 0 : (la < b.len - 1 ? -1 : 1);
+}
+
+// The record sources the kernels are instantiated for.  kSd: the record may carry structured data.  kOptional:
+// application_name and process_id are None, and level is None without a severity.  kLtsv: pairs are LtsvKey / LtsvVal
+// (composed keys, typed values), and the size pass writes the "Missing value" stop of every line.
+struct From5424 {
+    static constexpr bool kSd = true, kOptional = false, kLtsv = false;
+    using Key = Span;
+    using Val = Span;
+    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view(P, B, i, r); }
+    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.rows[2 * (size_t)i].z & 0xFFu; }
+    static __device__ __forceinline__ bool pair(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, uint32_t e, Key& k, Val& v) {
+        return load_pair(P, B, r, e, k, v);
+    }
+};
+struct From3164 {
+    static constexpr bool kSd = false, kOptional = true, kLtsv = false;
+    using Key = Span;
+    using Val = Span;
+    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_3164(P, B, i, r); }
+    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.col_meta[i] & 0xFFu; }
+    static __device__ __forceinline__ bool pair(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, uint32_t e, Key& k, Val& v) {
+        return load_pair(P, B, r, e, k, v);
+    }
+};
+struct FromLtsv {
+    static constexpr bool kSd = true, kOptional = true, kLtsv = true;
+    using Key = LtsvKey;
+    using Val = LtsvVal;
+    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_ltsv(P, B, i, r); }
+    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.col_meta[i] & 0xFFu; }
+    static __device__ __forceinline__ bool pair(const GelfEncodeParams& P, const ByteSource& B, const RecView&, uint32_t e, Key& k, Val& v) {
+        return load_pair_ltsv(P, B, e, k, v);
+    }
+};
+
+// ltsv_decoder.rs:99 prints "Missing value for name '{part}'" for every part without ':' the decode loop reached.  The
+// stop of line i, relative to its start: -1 when nothing was printed, else the end of the parts that were read — the
+// failing part's offset on an error row (fg_parse_ltsv.cu keeps it in full.x), the line's length + 1 otherwise.
+constexpr uint32_t kMissingValue = 0x02u;  // FG_FLAG_MISSING_VALUE
+__device__ __forceinline__ int32_t ltsv_stop(const GelfEncodeParams& P, int i) {
+    const uint32_t meta = P.col_meta[i], st = meta & 0xFFu;
+    if (!((meta >> 24) & kMissingValue) || st == FG_ES_INVALID_UTF8) return -1;  // a line that is not UTF-8 is not decoded
+    const int2 f = P.col_full[i];
+    return st ? f.x - P.offsets[i] : f.y + 1;
 }
 
 // static items (host-prepared, sorted by key, extras already override fixed keys of the same name)
@@ -275,7 +398,47 @@ struct SegList {
         push(v.p, v.len, true);
         lit(L_QUOTE, 1);
     }
+    // a number whose text does not exist yet (LTSV): the segment points at its 8 value bytes in the side table and holds
+    // its fg_ltsv_type as length; run_segments formats it when it reaches the segment
+    __device__ __forceinline__ void num(const unsigned long long* at, uint32_t tag) { push((const uint8_t*)at, (int)tag, false); }
 };
+
+// `"_` is already out; the rest of an LTSV pair: `name suffix":` and its value (ltsv_decoder.rs:131-193: a typed value is
+// an SDValue, written as serde_json writes Bool / F64 / I64 / U64)
+__device__ __forceinline__ void ltsv_pair(const GelfEncodeParams& P, SegList& L, const ByteSource& B, const LtsvKey& k, const LtsvVal& v) {
+    L.push(k.name.p, k.name.len, true);
+    L.push(k.suffix.p, k.suffix.len, true);
+    if (v.tag == 0u) {
+        L.lit(L_MID, 3);  // ":"
+        L.push(B.at((int)(uint32_t)v.v), (int)(v.v >> 32), true);
+        L.lit(L_QUOTE, 1);
+        return;
+    }
+    L.lit(L_MID, 2);  // ":
+    L.num(P.wentry_val + v.e, v.tag);
+}
+
+// serde_json 0.8 for the typed values of an LTSV record: Bool as true / false, F64 through dtoa (non-finite -> null),
+// I64 / U64 in decimal
+__device__ __forceinline__ int json_number(unsigned long long v, uint32_t tag, uint8_t* out) {
+    if (tag == 1u) {
+        const uint32_t w = v ? 0x65757274u : 0x736C6166u;  // "true" / "fals", low byte first
+        for (int k = 0; k < 4; ++k) out[k] = (uint8_t)(w >> (8 * k));
+        out[4] = 'e';
+        return v ? 4 : 5;
+    }
+    if (tag == 2u) return json_f64(__longlong_as_double((long long)v), out);
+    int n = 0;
+    if (tag == 3u && (long long)v < 0) {
+        out[n++] = '-';
+        v = 0ull - v;  // i64::MIN too
+    }
+    int d = 1;
+    for (unsigned long long t = v; t >= 10ull; t /= 10ull) ++d;
+    n += d;
+    for (int k = n - 1; d > 0; --k, --d, v /= 10ull) out[k] = (uint8_t)('0' + (uint32_t)(v % 10ull));
+    return n;
+}
 
 // SD pairs in BTreeMap order.  The pairs of a line are gathered once as (4-byte big-endian name prefix, row) and
 // insertion-sorted by prefix (full byte compare only on equal prefixes; stable, so of equal names the LAST one — the one
@@ -292,17 +455,22 @@ __device__ __forceinline__ uint32_t name_prefix(Span n) {
     return k;
 }
 
+// (keys and values of the source's type: Span for RFC5424, LtsvKey / LtsvVal for LTSV)
+template <class Src>
 struct PairCursor {
+    using Key = typename Src::Key;
+    using Val = typename Src::Val;
     PairRef pr[kLocalPairs];
     int np = 0, at = 0;
     bool many = false;
-    Span prev{nullptr, -1};
+    Key prev{nullptr, -1};
     bool have_prev = false;
 
     __device__ __forceinline__ void init(const GelfEncodeParams& P, const ByteSource& B, const RecView& r) {
         for (uint32_t e = r.first; e < r.first + r.count; ++e) {
-            Span nm, vl;
-            if (!load_pair(P, B, r, e, nm, vl)) continue;
+            Key nm;
+            Val vl;
+            if (!Src::pair(P, B, r, e, nm, vl)) continue;
             if (np == kLocalPairs) { many = true; break; }
             const uint32_t key = name_prefix(nm);
             int j = np++;
@@ -310,8 +478,9 @@ struct PairCursor {
                 const PairRef q = pr[j - 1];
                 bool after = q.key > key;
                 if (q.key == key) {
-                    Span qn, qv;
-                    load_pair(P, B, r, q.row, qn, qv);
+                    Key qn;
+                    Val qv;
+                    Src::pair(P, B, r, q.row, qn, qv);
                     after = cmp_names(qn, nm) > 0;
                 }
                 if (!after) break;
@@ -323,14 +492,15 @@ struct PairCursor {
         }
     }
     // next pair in key order with duplicates resolved; false when exhausted
-    __device__ __forceinline__ bool next(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, Span& bn, Span& bv) {
+    __device__ __forceinline__ bool next(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, Key& bn, Val& bv) {
         if (!many) {
             while (at < np) {
-                load_pair(P, B, r, pr[at].row, bn, bv);
+                Src::pair(P, B, r, pr[at].row, bn, bv);
                 ++at;
                 if (at < np && pr[at].key == pr[at - 1].key) {  // a later pair with the same name replaces this one
-                    Span nn, nv;
-                    load_pair(P, B, r, pr[at].row, nn, nv);
+                    Key nn;
+                    Val nv;
+                    Src::pair(P, B, r, pr[at].row, nn, nv);
                     if (cmp_names(nn, bn) == 0) continue;
                 }
                 return true;
@@ -339,8 +509,9 @@ struct PairCursor {
         }
         bool have = false;
         for (uint32_t e = r.first; e < r.first + r.count; ++e) {
-            Span nm, vl;
-            if (!load_pair(P, B, r, e, nm, vl)) continue;
+            Key nm;
+            Val vl;
+            if (!Src::pair(P, B, r, e, nm, vl)) continue;
             if (have_prev && cmp_names(nm, prev) <= 0) continue;
             if (!have || cmp_names(nm, bn) <= 0) {
                 bn = nm;
@@ -350,7 +521,7 @@ struct PairCursor {
         }
         return have;
     }
-    __device__ __forceinline__ void taken(Span bn) {
+    __device__ __forceinline__ void taken(Key bn) {
         prev = bn;
         have_prev = true;
     }
@@ -366,9 +537,10 @@ __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const 
                                                SegList& L) {
     if (live) L.lit(L_OPEN, 1);
     bool first = true;
-    PairCursor pc;
+    PairCursor<Src> pc;
     if (Src::kSd && live) pc.init(P, B, r);
-    Span bn{nullptr, 0}, bv{nullptr, 0};
+    typename Src::Key bn{nullptr, 0};
+    typename Src::Val bv{};
     bool have = Src::kSd && live && pc.next(P, B, r, bn, bv);
     for (int si = 0; si <= P.n_static; ++si) {  // warp-uniform; si == n_static: the pairs after the last static item
         const bool tail = si == P.n_static;
@@ -382,10 +554,14 @@ __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const 
             if (emit) {
                 L.lit(L_PAIR + (first ? 1 : 0), first ? 2 : 3);  // ,"_
                 first = false;
-                L.push(bn.p, bn.len, true);
-                L.lit(L_MID, 3);  // ":"
-                L.push(bv.p, bv.len, true);
-                L.lit(L_QUOTE, 1);
+                if constexpr (Src::kLtsv) {
+                    ltsv_pair(P, L, B, bn, bv);
+                } else {
+                    L.push(bn.p, bn.len, true);
+                    L.lit(L_MID, 3);  // ":"
+                    L.push(bv.p, bv.len, true);
+                    L.lit(L_QUOTE, 1);
+                }
                 pc.taken(bn);
                 have = pc.next(P, B, r, bn, bv);
             }
@@ -452,17 +628,30 @@ __device__ __forceinline__ uint32_t json_escape_flags4(uint32_t w) {
 
 // The warp-uniform loop: per lane and iteration FOUR output bytes when the segment has them and none needs an escape, else
 // one.  `live` = this lane has a record to emit.  (One byte per iteration spends the loop's bookkeeping on every byte.)
-template <class Sink>
+// kNum (Sink = NumSink): the list may hold number segments, formatted into `text` when the loop enters them (segments are
+// consumed in order, so one buffer serves all the numbers of a record).
+template <class Sink, bool kNum = false>
 __device__ __forceinline__ void run_segments(const SegList& L, bool live, Sink& s) {
     int si = 0, k = 0, len = 0;
     bool esc = false;
     const uint8_t* p = nullptr;
     uint32_t pending = 0;
     bool more = live && L.n > 0;
+    uint8_t text[kNum ? 32 : 1];
+    auto enter_number = [&]() {
+        if constexpr (kNum) {
+            const unsigned long long* v = reinterpret_cast<const unsigned long long*>(p);
+            if (v >= s.vals && v < s.vals + s.cap) {  // no byte segment points into the value column
+                len = json_number(*v, (uint32_t)len, text);
+                p = text;
+            }
+        }
+    };
     if (more) {
         p = L.s[0].p;
         len = L.s[0].len & ~kEscBit;
         esc = L.s[0].len < 0;
+        enter_number();
     }
     while (__any_sync(0xFFFFFFFFu, more)) {
         if (more) {
@@ -494,6 +683,7 @@ __device__ __forceinline__ void run_segments(const SegList& L, bool live, Sink& 
                     len = L.s[si].len & ~kEscBit;
                     esc = L.s[si].len < 0;
                     k = 0;
+                    enter_number();
                 } else {
                     more = false;
                 }
@@ -511,7 +701,12 @@ __device__ __forceinline__ void emit_record(const GelfEncodeParams& P, const Byt
     for (;;) {
         L.reset(skip);
         build_segments<Src>(P, B, r, live, num, L);
-        run_segments(L, live, s);
+        if constexpr (Src::kLtsv) {
+            NumSink<Sink> ns{s, P.wentry_val, P.wentry_cap};
+            run_segments<NumSink<Sink>, true>(L, live, ns);
+        } else {
+            run_segments(L, live, s);
+        }
         skip += kMaxSegs;
         if (!__any_sync(0xFFFFFFFFu, live && L.idx > skip)) break;
     }
@@ -600,6 +795,7 @@ __global__ void __launch_bounds__(kEncLines) gelf_size_kernel(const __grid_const
     if (!valid) return;
     P.lens[i] = r.ok ? s.n : 0ull;
     P.status[i] = (uint8_t)Src::status(P, i);
+    if constexpr (Src::kLtsv) P.ltsv_stop[i] = ltsv_stop(P, i);
 }
 
 // chunk totals: base[k + 1] = base[k] + bytes of this chunk (one thread)
@@ -654,11 +850,13 @@ cudaError_t launch_src(const GelfEncodeParams& p, void* d_scan_temp, size_t scan
 
 }  // namespace
 
-// both sources get the same staging limit: launch_encode clamps every tile to it
+// every source gets the same staging limit: launch_encode clamps every tile to it
 cudaError_t configure_gelf_encode(int max_tile_bytes) {
     cudaError_t e = configure_src<From5424>(max_tile_bytes);
     if (e != cudaSuccess) return e;
-    return configure_src<From3164>(max_tile_bytes);
+    e = configure_src<From3164>(max_tile_bytes);
+    if (e != cudaSuccess) return e;
+    return configure_src<FromLtsv>(max_tile_bytes);
 }
 
 size_t gelf_scan_temp_bytes(int n) {
@@ -671,6 +869,7 @@ cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_
     if (p.n <= 0) return cudaSuccess;
     switch (fmt) {
         case 0: return launch_src<From5424>(p, d_scan_temp, scan_temp_bytes, stream);
+        case 1: return launch_src<FromLtsv>(p, d_scan_temp, scan_temp_bytes, stream);
         case 3: return launch_src<From3164>(p, d_scan_temp, scan_temp_bytes, stream);
         default: return cudaErrorInvalidValue;
     }

@@ -138,7 +138,7 @@ cudaError_t launch_parse5424(const Parse5424Params& p, cudaStream_t stream, cuda
 cudaError_t configure_parse5424(int max_tile_bytes);
 int parse5424_smem_bytes(int tile_bytes);
 
-// ---- fused GELF encoder over the RFC5424 or RFC3164 results (fg_gelf_encode.cu) ---------------------------------------
+// ---- fused GELF encoder over the RFC5424, RFC3164 or LTSV results (fg_gelf_encode.cu) ---------------------------------
 struct GelfEncodeParams {
     const uint8_t* bytes;
     const int32_t* offsets;  // [n+1], element 0 = first line of this launch
@@ -166,17 +166,24 @@ struct GelfEncodeParams {
     const uint32_t* bad_offsets;
     uint32_t entry_cap, wide_cap, wentry_cap;  // a table that overflowed is not read (the batch is redone after a regrow)
     int32_t tile_bytes;                        // staging tile of the two kernels (dynamic shared memory)
-    // RFC3164 source: the row columns parse3164_kernel wrote for these lines (element 0 = first line of this launch);
-    // spans are absolute in `bytes`, except a message flagged FG_FLAG_MSG_ARENA, whose offset indexes `arena`
-    const double* r3_ts;
-    const uint32_t* r3_meta;
-    const int2* r3_host;
-    const int2* r3_msg;
-    const int2* r3_full;
+    // RFC3164 and LTSV sources: the row columns the parse kernel wrote for these lines (element 0 = first line of this
+    // launch); spans are absolute in `bytes`, except an RFC3164 message flagged FG_FLAG_MSG_ARENA, whose offset indexes
+    // `arena`
+    const double* col_ts;
+    const uint32_t* col_meta;
+    const int2* col_host;
+    const int2* col_msg;
+    const int2* col_full;
     uint32_t arena_cap;
+    // LTSV source: sd = {first row, count} of the line's pairs in wentry_*; the type suffixes (LtsvDeviceConfig.suffix,
+    // suffix_off); stop[i] receives where the decoder stopped printing "Missing value" lines (fg_encoded_ltsv_stops)
+    const int2* col_sd;
+    const uint8_t* ltsv_suffix;
+    int32_t ltsv_suffix_off[6];
+    int32_t* ltsv_stop;
 };
 cudaError_t configure_gelf_encode(int max_tile_bytes);
-// fmt: the decoder whose results the encoder reads (0 = RFC5424, 3 = RFC3164)
+// fmt: the decoder whose results the encoder reads (0 = RFC5424, 1 = LTSV, 3 = RFC3164)
 cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
 size_t gelf_scan_temp_bytes(int n);
 

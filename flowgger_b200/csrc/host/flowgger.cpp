@@ -182,6 +182,7 @@ CudaBatchDecoder::CudaBatchDecoder(fg_format fmt, const LtsvConfig& ltsv, const 
     cfg.chunk_lines = opt.chunk_lines;
     cfg.rfc3164_year = opt.rfc3164_year;
     cfg.tzdir = opt.tzdir.empty() ? nullptr : opt.tzdir.c_str();
+    cfg.input_format = (int32_t)fmt;
     std::vector<const char*> names;
     std::vector<int32_t> types;
     for (const auto& kv : ltsv.schema) {
@@ -242,6 +243,11 @@ void CudaBatchDecoder::decode_encode_gelf(const uint8_t* bytes, const int32_t* o
     set_gelf_extra(extra);
     const int rc = fg_decode_encode_gelf(ctx_, fmt_, bytes, offsets, n, out);
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_encode_gelf: ") + fg_last_error(ctx_));
+}
+
+const int32_t* CudaBatchDecoder::encoded_ltsv_stops() const {
+    const int32_t* stop = nullptr;
+    return fmt_ == FG_FMT_LTSV && fg_encoded_ltsv_stops(ctx_, &stop) == FG_OK ? stop : nullptr;
 }
 
 bool CudaBatchDecoder::try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
@@ -398,6 +404,18 @@ static DecodeResult materialize_5424(const fg_batch_out& out, const uint8_t* byt
     return r;
 }
 
+void ltsv_missing_values(const uint8_t* bytes, int32_t lo, int32_t hi, int32_t stop, std::vector<std::string>& out) {
+    for (int32_t a = lo;;) {
+        int32_t b = a;
+        while (b < hi && bytes[b] != '\t') ++b;
+        if (a >= stop) break;
+        std::string_view part((const char*)bytes + a, (size_t)(b - a));
+        if (part.find(':') == std::string_view::npos) out.push_back("Missing value for name '" + std::string(part) + "'");
+        if (b >= hi) break;
+        a = b + 1;
+    }
+}
+
 DecodeResult materialize_record(fg_format fmt, const std::string* suffix, const fg_batch_out& out, const uint8_t* bytes,
                                 int32_t line_lo, int32_t line_hi, int32_t i, std::vector<std::string>* side_effects) {
     if (fmt == FG_FMT_RFC5424) return materialize_5424(out, bytes, line_lo, i);
@@ -405,21 +423,8 @@ DecodeResult materialize_record(fg_format fmt, const std::string* suffix, const 
     const uint32_t meta = out.meta[i];
     const uint32_t status = FG_META_STATUS(meta), flags = FG_META_FLAGS(meta);
     if (side_effects && (flags & FG_FLAG_MISSING_VALUE)) {
-        // println! at ltsv_decoder.rs:99 for every tab-separated part without ':' that the decode loop
-        // reached: all parts when Ok / post-loop error, else the parts before the failing one.
-        const int32_t lo = line_lo, hi = line_hi;
-        const int32_t stop = status ? out.full_msg[i].off : hi + 1;
-        int32_t a = lo;
-        for (;;) {
-            int32_t b = a;
-            while (b < hi && bytes[b] != '\t') ++b;
-            if (a >= stop) break;
-            std::string_view part((const char*)bytes + a, (size_t)(b - a));
-            if (part.find(':') == std::string_view::npos)
-                side_effects->push_back("Missing value for name '" + std::string(part) + "'");
-            if (b >= hi) break;
-            a = b + 1;
-        }
+        // all parts when Ok / post-loop error, else the parts before the failing one
+        ltsv_missing_values(bytes, line_lo, line_hi, status ? out.full_msg[i].off : line_hi + 1, *side_effects);
     }
     if (status) {
         r.err = fg_error_string(fmt, status);
@@ -530,8 +535,16 @@ void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
         // decode + encode on the device (line_splitter.rs:50-52 fused): only the encoded records come back
         fg_encoded_out eo;
         gpu->decode_encode_gelf(bytes, offsets_.data(), n, fused_->extra(), &eo);
+        const int32_t* stops = gpu->encoded_ltsv_stops();
+        std::vector<std::string> fx;
         for (int32_t i = 0; i < n; ++i) {
             invalid(i);
+            if (stops && stops[i] >= 0) {
+                fx.clear();
+                const int32_t lo = offsets_[(size_t)i];
+                ltsv_missing_values(bytes, lo, offsets_[(size_t)i + 1], lo + stops[i], fx);
+                for (const auto& s : fx) out_ << s << "\n";
+            }
             if (eo.status[i] == 0) tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
             else report(fg_error_string(gpu->format(), eo.status[i]),
                         std::string_view((const char*)bytes + offsets_[(size_t)i], (size_t)(offsets_[(size_t)i + 1] - offsets_[(size_t)i])));
@@ -658,13 +671,20 @@ class BlockSplitter {
             fg_encoded_out eo;
             const int32_t* lines;
             if (!gpu->try_split_decode_encode_gelf(p, n, framing_, fused_->extra(), &eo, &lines)) return false;
+            const int32_t* stops = gpu->encoded_ltsv_stops();
+            std::vector<std::string> fx;
             for (int32_t i = 0; i < eo.n; ++i) {
+                int32_t lo, hi;
+                split_extent(lines, p, i, lo, hi, framing_);
+                if (stops && stops[i] >= 0) {
+                    fx.clear();
+                    ltsv_missing_values(p, lo, hi, lines[i] + stops[i], fx);
+                    for (const auto& s : fx) out_ << s << "\n";
+                }
                 if (eo.status[i] == 0) {
                     tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
                     continue;
                 }
-                int32_t lo, hi;
-                split_extent(lines, p, i, lo, hi, framing_);
                 reject(fmt, eo.status[i], fg_error_string(fmt, eo.status[i]), p, lo, hi);
             }
             return true;
@@ -1140,10 +1160,11 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
 }
 
 // BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or BatchingSyslenSplitter (framing 2, through
-// RecordBatcher) with output.format = "gelf" (fused decode + encode): text in, one JSON record per line out
+// RecordBatcher) with output.format = "gelf" (fused decode + encode): text in, one JSON record per line, stderr and
+// stdout text out
 int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
                           const char* const* keys, const char* const* vals, uint8_t** out_records, int64_t* out_records_len,
-                          uint8_t** out_stderr, int64_t* out_stderr_len, int framing) {
+                          uint8_t** out_stderr, int64_t* out_stderr_len, int framing, uint8_t** out_stdout, int64_t* out_stdout_len) {
     struct Shared : Decoder {
         std::shared_ptr<CudaBatchDecoder> b;
         DecodeResult decode(std::string_view) const override { return {}; }
@@ -1176,6 +1197,7 @@ int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max
     };
     give(records, out_records, out_records_len);
     give(es.str(), out_stderr, out_stderr_len);
+    give(os.str(), out_stdout, out_stdout_len);
     return 0;
 }
 

@@ -122,6 +122,9 @@ class CudaBatchDecoder {
     bool try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
                                       const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out,
                                       const int32_t** line_offsets);
+    // after one of the two fused calls on an LTSV context: where each record's "Missing value" lines stop
+    // (fg_encoded_ltsv_stops, for ltsv_missing_values); nullptr for other formats
+    const int32_t* encoded_ltsv_stops() const;
 
    private:
     void set_gelf_extra(const std::vector<std::pair<std::string, std::string>>& extra);
@@ -180,12 +183,13 @@ class Encoder {
 
 // encoder/gelf_encoder.rs:10-48: output.format = "gelf".  The encoder runs FUSED with the decoder on the GPU
 // (fg_decode_encode_gelf) for the input formats fuses_with() accepts: the batching splitters and RecordBatcher recognise
-// this type and never materialise Records for them.
+// this type and never materialise Records for them (for LTSV they print the decoder's "Missing value" lines from
+// fg_encoded_ltsv_stops).
 class CudaGelfEncoder : public Encoder {
    public:
     explicit CudaGelfEncoder(std::vector<std::pair<std::string, std::string>> extra = {}) : extra_(std::move(extra)) {}
     // the decoders whose device-resident results the fused encoder reads (fg_decode_encode_gelf)
-    static bool fuses_with(fg_format fmt) { return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164; }
+    static bool fuses_with(fg_format fmt) { return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || fmt == FG_FMT_LTSV; }
     // a lone host-side Record cannot be encoded: there is no CPU encoder behind this interface
     bool encode(Record&&, std::vector<uint8_t>&, const char** err) const override {
         if (err) *err = "GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)";
@@ -309,6 +313,9 @@ class MultiGpuBatchDecoder {
 // five LTSV type suffixes (may be null for other formats).  Pure function of the result arrays: no device, no context.
 DecodeResult materialize_record(fg_format fmt, const std::string* suffix, const fg_batch_out& out, const uint8_t* bytes,
                                 int32_t line_lo, int32_t line_hi, int32_t i, std::vector<std::string>* side_effects);
+// The println! of ltsv_decoder.rs:99 for the LTSV record bytes[lo, hi): "Missing value for name '{part}'" for every
+// tab-separated part without ':' that starts before `stop` (absolute; hi + 1 = every part), appended to `out` in order
+void ltsv_missing_values(const uint8_t* bytes, int32_t lo, int32_t hi, int32_t stop, std::vector<std::string>& out);
 uint32_t row_meta(const fg_batch_out& out, int32_t i);
 
 // helpers shared with tests

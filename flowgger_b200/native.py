@@ -105,6 +105,7 @@ def load_cuda() -> C.CDLL:
         L.fg_decode_encode_gelf.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(FgEncodedOut)]
         L.fg_split_decode_encode_gelf.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.POINTER(FgEncodedOut),
                                                   C.POINTER(C.POINTER(C.c_int32))]
+        L.fg_encoded_ltsv_stops.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
         _cuda = L
     return _cuda
 
@@ -139,7 +140,8 @@ def load_host() -> C.CDLL:
         L.fgh_clone_decode_threads.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.c_int,
                                                C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_char_p, C.c_int]
         L.fgh_splitter_run_gelf.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int64, C.c_int, C.POINTER(C.c_char_p),
-                                            C.POINTER(C.c_char_p)] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 2 + [C.c_int]
+                                            C.POINTER(C.c_char_p)] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 2 + [C.c_int] + [
+                                            C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
         L.fgh_splitter_run.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int64, C.c_int32, C.c_int64] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         _host = L
     return _host
@@ -354,15 +356,19 @@ class BatchDecoder:
         self._check(self.L.fg_set_gelf_extra(self.ctx, len(ex), keys, vals), "fg_set_gelf_extra")
 
     def decode_encode_gelf(self, data: np.ndarray, offsets: np.ndarray, copy: bool = True):
-        """decode + GelfEncoder::encode fused on the device, for a decoder of FMT_RFC5424 or FMT_RFC3164 (LTSV and GELF
-        raise): (JSON bytes, int64 offsets[n+1], status uint8[n], kernel ms).  An RFC3164 record has no application_name,
-        process_id or sd_id, "level" only when the line has a <PRI>, and always a "short_message" (possibly "").
-        With copy=False the arrays are views of the context's pinned buffers (valid until the next call)."""
+        """decode + GelfEncoder::encode fused on the device, for a decoder of FMT_RFC5424, FMT_RFC3164 or FMT_LTSV (GELF
+        raises): (JSON bytes, int64 offsets[n+1], status uint8[n], kernel ms).  An RFC3164 record has no application_name,
+        process_id or sd_id, "level" only when the line has a <PRI>, and always a "short_message" (possibly "").  An LTSV
+        record has no application_name, process_id or sd_id, one "_" + name (+ type suffix) key per pair with typed
+        values as JSON bools / numbers, and "-" as short_message without a `message` part; ltsv_stops() gives its
+        "Missing value" lines.  With copy=False the arrays are views of the context's pinned buffers (valid until the
+        next call)."""
         assert data.dtype == np.uint8 and offsets.dtype == np.int32
         out = FgEncodedOut()
         n = len(offsets) - 1
         self._keep = (data, offsets)
         self._check(self.L.fg_decode_encode_gelf(self.ctx, self.fmt, _ptr(data), _ptr(offsets), n, C.byref(out)), "fg_decode_encode_gelf")
+        self._last_encoded_n = n
         offs = np.ctypeslib.as_array(out.offsets, shape=(n + 1,))
         total = int(offs[-1]) if n else 0
         buf = np.ctypeslib.as_array(out.bytes, shape=(max(total, 1),))[:total]
@@ -372,7 +378,7 @@ class BatchDecoder:
         return buf, offs, status, out.kernel_ms
 
     def split_decode_encode_gelf(self, stream: np.ndarray, framing: int = 0, copy: bool = True):
-        """Framing (0 = "line", 1 = "nul") + UTF-8 validation + decode (FMT_RFC5424 or FMT_RFC3164) + GelfEncoder::encode
+        """Framing (0 = "line", 1 = "nul") + UTF-8 validation + decode (FMT_RFC5424, FMT_RFC3164 or FMT_LTSV) + GelfEncoder::encode
         of a raw byte stream, all on the device: (JSON bytes, int64 offsets[n+1], status uint8[n], record starts
         int32[n+1] in `stream` with their terminators, kernel ms).  A record that is not UTF-8 has status 76
         ("Invalid UTF-8 input") and an empty JSON record.
@@ -384,6 +390,7 @@ class BatchDecoder:
         self._check(self.L.fg_split_decode_encode_gelf(self.ctx, self.fmt, framing, _ptr(stream), len(stream), C.byref(out), C.byref(lo)),
                     "fg_split_decode_encode_gelf")
         n = out.n
+        self._last_encoded_n = n
         offs = np.ctypeslib.as_array(out.offsets, shape=(n + 1,))
         total = int(offs[-1]) if n else 0
         buf = np.ctypeslib.as_array(out.bytes, shape=(max(total, 1),))[:total]
@@ -392,6 +399,15 @@ class BatchDecoder:
         if copy:
             return buf.tobytes(), offs.copy(), status.copy(), lines.copy(), out.kernel_ms
         return buf, offs, status, lines, out.kernel_ms
+
+    def ltsv_stops(self) -> np.ndarray:
+        """After decode_encode_gelf / split_decode_encode_gelf on an LTSV decoder: int32[n], -1 where the decoder printed
+        nothing, else the offset from the record's start up to which its parts were read (fg_encoded_ltsv_stops); every
+        part before it without ':' printed "Missing value for name '<part>'"."""
+        p = C.POINTER(C.c_int32)()
+        self._check(self.L.fg_encoded_ltsv_stops(self.ctx, C.byref(p)), "fg_encoded_ltsv_stops")
+        n = self._last_encoded_n
+        return np.ctypeslib.as_array(p, shape=(n,)).copy() if n else np.zeros(0, np.int32)
 
     def split_decode(self, stream: np.ndarray) -> BatchResult:
         """Framing + UTF-8 validation + decode of a raw newline-terminated byte stream, all on the device."""
@@ -554,26 +570,26 @@ def clone_decode_threads(fmt: int, lines: list[bytes], nthreads: int = 2, device
 
 
 def splitter_run_gelf(dec: "BatchDecoder", text: bytes, extra: dict[str, str] | None = None, max_lines: int = 1 << 16,
-                      max_bytes: int = 16 << 20, framing: int = 0) -> tuple[bytes, bytes]:
+                      max_bytes: int = 16 << 20, framing: int = 0, stdout: bool = False) -> tuple[bytes, ...]:
     """BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or BatchingSyslenSplitter (framing 2: records
-    framed on the host and batched by RecordBatcher) with input.format = rfc5424 or rfc3164 (the decoder's format) and
-    output.format = gelf (decode and encode fused on the GPU, framing too for 0 and 1): returns (JSON records separated
-    by newlines, stderr text)."""
+    framed on the host and batched by RecordBatcher) with input.format = rfc5424, rfc3164 or ltsv (the decoder's format)
+    and output.format = gelf (decode and encode fused on the GPU, framing too for 0 and 1): returns (JSON records
+    separated by newlines, stderr text), and with stdout=True also the stdout text (LTSV's "Missing value" lines)."""
     H = load_host()
     ex = list((extra or {}).items())
     keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])
     vals = (C.c_char_p * max(len(ex), 1))(*[v.encode() for _, v in ex])
-    ps = [C.c_void_p() for _ in range(2)]
-    ns = [C.c_int64() for _ in range(2)]
+    ps = [C.c_void_p() for _ in range(3)]
+    ns = [C.c_int64() for _ in range(3)]
     rc = H.fgh_splitter_run_gelf(dec._h, text, len(text), max_lines, max_bytes, len(ex), keys, vals, C.byref(ps[0]), C.byref(ns[0]),
-                                 C.byref(ps[1]), C.byref(ns[1]), framing)
+                                 C.byref(ps[1]), C.byref(ns[1]), framing, C.byref(ps[2]), C.byref(ns[2]))
     if rc != 0:
         raise RuntimeError("splitter failed")
     out = []
     for p, n in zip(ps, ns):
         out.append(C.string_at(p, n.value))
         H.fgh_free(p)
-    return tuple(out)
+    return tuple(out) if stdout else tuple(out[:2])
 
 
 def splitter_run(dec: "BatchDecoder", text: bytes, max_lines: int = 1 << 16, max_bytes: int = 16 << 20,

@@ -153,6 +153,10 @@ typedef struct fg_config {
      *   /usr/share/zoneinfo.  Read on the first RFC3164 call; fg_set_tz_table replaces it with the caller's own table. */
     int32_t rfc3164_year;
     const char* tzdir;
+    /* input.format the context is created for (mod.rs:413-422: the reference builds one decoder per configuration);
+     * 0 = rfc5424.  Decoding takes the format per call; the fused GELF encoder takes LTSV input only on a context created
+     * for LTSV, because it writes the pair keys with that context's ltsv_suffixes. */
+    int32_t input_format;
 } fg_config;
 
 /* Columnar result of one batch.  All pointers are host pointers owned by the
@@ -250,8 +254,8 @@ int fg_flush_l2(fg_ctx* ctx); /* writes a >L2-sized scratch buffer */
 
 /* ---- decode + encode fused on the device (SURVEY.md 8(f) N2) ------------------------------------------------------
  * The reference calls Encoder::encode right after Decoder::decode for every record (splitter/line_splitter.rs:50-52).
- * For output.format = "gelf" with input.format = "rfc5424" (the default pair) or "rfc3164" both stages run on the GPU
- * and only the encoded records come back:
+ * For output.format = "gelf" with input.format = "rfc5424" (the default pair), "rfc3164" or "ltsv" both stages run on
+ * the GPU and only the encoded records come back:
  *     GelfEncoder::new(&Config)   encoder/gelf_encoder.rs:29-48   -> fg_set_gelf_extra (output.gelf_extra)
  *     Encoder::encode(Record)     encoder/gelf_encoder.rs:59-115, encoder/mod.rs:54-56 -> fg_decode_encode_gelf
  * Record i is bytes[offsets[i], offsets[i+1]) — exactly the Vec<u8> the reference's encode returns (serde_json 0.8
@@ -259,7 +263,12 @@ int fg_flush_l2(fg_ctx* ctx); /* writes a >L2-sized scratch buffer */
  * status[i] != 0 (fg_error_string) and an empty record.  An RFC3164 record has no application_name, process_id or sd_id
  * (the Record holds None for them; a gelf_extra of that key is still written), "level" only when the line has a <PRI>,
  * and "short_message" always (possibly ""), as rfc3164_decoder.rs builds it.  The year of a timestamp without one is
- * fixed at the start of each call (fg_set_rfc3164_year).  LTSV and GELF input -> FG_E_ARG. */
+ * fixed at the start of each call (fg_set_rfc3164_year).  An LTSV record (ltsv_decoder.rs:87-221) has no
+ * application_name, process_id or sd_id, "level" only when the line has a `level` part, "short_message" "-" without a
+ * `message` part and "" for `message:`, and one "_" + name (+ the type's suffix, input.ltsv_suffixes) key per pair: a
+ * later pair of the same key replaces an earlier one, and a schema-typed value is written as a JSON bool or number
+ * (non-finite f64 -> null).  GELF input, and LTSV input on a context not created for LTSV
+ * (fg_config.input_format), -> FG_E_ARG. */
 typedef struct fg_encoded_out {
     int32_t n;
     const uint8_t* bytes;     /* concatenated records */
@@ -269,17 +278,25 @@ typedef struct fg_encoded_out {
     float total_ms;
 } fg_encoded_out;
 int fg_set_gelf_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
-int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 */, const uint8_t* bytes, const int32_t* offsets,
-                          int32_t n, fg_encoded_out* out);
-/* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424 or RFC3164
- * decode -> GelfEncoder::encode, all on the device; only the encoded records and the record extents come back.
+int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV */, const uint8_t* bytes,
+                          const int32_t* offsets, int32_t n, fg_encoded_out* out);
+/* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424, RFC3164 or
+ * LTSV decode -> GelfEncoder::encode, all on the device; only the encoded records and the record extents come back.
  * Record i is out->bytes[out->offsets[i], out->offsets[i+1]); out->status[i] is 0, a decoder status, or the framing status
  * whose fg_error_string is "Invalid UTF-8 input" (empty record).  *line_offsets ([n+1], starts in `stream`, each record
  * still carrying its terminator, like fg_batch_out.line_offsets) stays valid until the next call on the context.
- * Errors: LTSV or GELF input or an unknown framing -> FG_E_ARG; nbytes > max_batch_bytes or more records than
+ * Errors: GELF input, LTSV input on a context not created for LTSV, or an unknown framing -> FG_E_ARG; nbytes > max_batch_bytes or more records than
  * max_batch_lines -> FG_E_CAPACITY (the context stays usable). */
-int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 */, fg_framing framing, const uint8_t* stream,
-                                int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
+int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV */, fg_framing framing,
+                                const uint8_t* stream, int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
+/* The one side effect of LTSVDecoder::decode, println!("Missing value for name '{}'") for every tab-separated part
+ * without ':' that the decode loop reached (ltsv_decoder.rs:99), for the records of the last fused call on an LTSV
+ * context.  *stop ([out->n], valid until the next call on the context): -1 when record i printed nothing; else the offset,
+ * relative to the record's start (offsets[i], or *line_offsets[i] in split mode), up to which its parts were read: the
+ * failing part's offset on an error row, the record's length (without its terminator) + 1 otherwise.  Every part of the
+ * record that starts before that offset and holds no ':' prints one line, in order.  A record that is not UTF-8 has -1.
+ * Returns FG_E_ARG when the last fused call was not on LTSV input or failed. */
+int fg_encoded_ltsv_stops(const fg_ctx* ctx, const int32_t** stop);
 
 /* the reference's Err(&'static str) for a row status (0 -> NULL) */
 const char* fg_error_string(fg_format fmt, uint32_t status);

@@ -123,6 +123,7 @@ impl CudaDecoder {
         cfg.max_batch_lines = max_lines;
         cfg.rfc3164_year = 0;
         cfg.tzdir = spec.tzdir.as_ref().map_or(ptr::null(), |s| s.as_ptr());
+        cfg.input_format = fmt as i32;
         cfg.ltsv_has_schema = spec.has_schema as i32;
         cfg.ltsv_schema_len = spec.names.len() as i32;
         cfg.ltsv_schema_names = name_ptrs.as_ptr();
@@ -216,11 +217,12 @@ impl CudaDecoder {
     }
 
     /// Framing + UTF-8 validation + decode + `GelfEncoder::encode` of a raw stream on the device
-    /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424" or "rfc3164", see `fuses_with_gelf`): `f(line, Ok(json) |
-    /// Err(error))` in stream order, `line`
-    /// without its terminator.  false (nothing decoded) when the stream does not fit the context.
-    pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>)>(&self, stream: &[u8], extra: &[(String, String)],
-                                                                                   mut f: F) -> bool {
+    /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424", "rfc3164" or "ltsv", see `fuses_with_gelf`):
+    /// `f(line, Ok(json) | Err(error), side)` in stream order, `line` without its terminator, `side` the decoder's
+    /// println! lines for it (LTSV's "Missing value" lines, from `fg_encoded_ltsv_stops`).  false (nothing decoded) when
+    /// the stream does not fit the context.
+    pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String])>(&self, stream: &[u8],
+                                                                                             extra: &[(String, String)], mut f: F) -> bool {
         let mut ctx = self.ctx.lock().unwrap();
         if ctx.extra.as_deref() != Some(extra) {
             let keys: Vec<CString> = extra.iter().map(|(k, _)| CString::new(k.as_str()).unwrap()).collect();
@@ -245,13 +247,24 @@ impl CudaDecoder {
         }
         let n = out.n as usize;
         let offs = unsafe { std::slice::from_raw_parts(lines, n + 1) };
+        let mut stops: *const i32 = ptr::null();
+        if ctx.fmt == fg_format_FG_FMT_LTSV {
+            assert_eq!(unsafe { fg_encoded_ltsv_stops(ctx.raw, &mut stops) }, 0);
+        }
+        let mut side = Vec::new();
         for i in 0..n {
             let (lo, hi) = line_extent(stream, offs, i);
+            side.clear();
+            let stop = if stops.is_null() { -1 } else { unsafe { *stops.add(i) } };
+            if stop >= 0 {
+                // a record with a stop passed the UTF-8 check
+                missing_values(unsafe { std::str::from_utf8_unchecked(&stream[lo..hi]) }, stop as usize, &mut side);
+            }
             let (st, a, b) = unsafe { (*out.status.add(i), *out.offsets.add(i) as usize, *out.offsets.add(i + 1) as usize) };
             if st == 0 {
-                f(&stream[lo..hi], Ok(unsafe { std::slice::from_raw_parts(out.bytes.add(a), b - a) }));
+                f(&stream[lo..hi], Ok(unsafe { std::slice::from_raw_parts(out.bytes.add(a), b - a) }), &side);
             } else {
-                f(&stream[lo..hi], Err(error_str(ctx.fmt, st as u32)));
+                f(&stream[lo..hi], Err(error_str(ctx.fmt, st as u32)), &side);
             }
         }
         true
@@ -429,6 +442,17 @@ unsafe fn materialize_5424(ctx: &Ctx, out: &fg_batch_out, bytes: &[u8], line_lo:
     })
 }
 
+/// The println! of ltsv_decoder.rs:99: "Missing value for name '{part}'" for every tab-separated part of `line` without
+/// ':' that starts before `stop` (relative to the line; `line.len() + 1` = every part)
+fn missing_values(line: &str, stop: usize, side: &mut Vec<String>) {
+    let mut a = 0;
+    for part in line.split('\t') {
+        if a >= stop { break; }
+        if !part.contains(':') { side.push(format!("Missing value for name '{}'", part)); }
+        a += part.len() + 1;
+    }
+}
+
 fn materialize_ext(ctx: &Ctx, out: &fg_batch_out, bytes: &[u8], line_lo: i32, line_hi: i32, i: usize, side: &mut Vec<String>) -> Result<Record, &'static str> {
     unsafe {
         if !out.rows5424.is_null() {
@@ -438,15 +462,10 @@ fn materialize_ext(ctx: &Ctx, out: &fg_batch_out, bytes: &[u8], line_lo: i32, li
         let status = meta & 0xFF;
         let flags = (meta >> 24) & 0xFF;
         if flags & FG_FLAG_MISSING_VALUE != 0 {
-            // println! at ltsv_decoder.rs:99 for every part without ':' that the decode loop reached
+            // all parts when Ok / post-loop error, else the parts before the failing one
             let (lo, hi) = (line_lo as usize, line_hi as usize);
             let stop = if status != 0 { (*out.full_msg.add(i)).off as usize } else { hi + 1 };
-            let mut a = lo;
-            for part in span(bytes, fg_span { off: lo as i32, len: (hi - lo) as i32 }).split('\t') {
-                if a >= stop { break; }
-                if !part.contains(':') { side.push(format!("Missing value for name '{}'", part)); }
-                a += part.len() + 1;
-            }
+            missing_values(span(bytes, fg_span { off: lo as i32, len: (hi - lo) as i32 }), stop - lo, side);
         }
         if status != 0 {
             let s = CStr::from_ptr(fg_error_string(ctx.fmt, status));
@@ -564,13 +583,14 @@ impl<T: Read> Splitter<T> for BatchingLineSplitter {
 /// The `input.format` values whose decoder runs fused with the GELF encoder on the device (`fg_decode_encode_gelf`,
 /// `fg_split_decode_encode_gelf`); `FusedGelfLineSplitter` takes a `CudaDecoder` of one of them.
 pub fn fuses_with_gelf(input_format: &str) -> bool {
-    matches!(input_format, "rfc5424" | "rfc3164")
+    matches!(input_format, "rfc5424" | "rfc3164" | "ltsv")
 }
 
-/// `output.format = "gelf"` with `input.format = "rfc5424"` or `"rfc3164"` (`fuses_with_gelf`): framing, the UTF-8 check,
-/// decode AND encode run on the device (`fg_split_decode_encode_gelf`, replaces BufRead::lines + Decoder::decode +
-/// GelfEncoder::encode of line_splitter.rs:17-52); it reads raw blocks like `BatchingLineSplitter` and only the encoded
-/// records come back.  An RFC3164 context fixes the year of year-less timestamps at the start of each call.
+/// `output.format = "gelf"` with `input.format = "rfc5424"`, `"rfc3164"` or `"ltsv"` (`fuses_with_gelf`): framing, the
+/// UTF-8 check, decode AND encode run on the device (`fg_split_decode_encode_gelf`, replaces BufRead::lines +
+/// Decoder::decode + GelfEncoder::encode of line_splitter.rs:17-52); it reads raw blocks like `BatchingLineSplitter` and
+/// only the encoded records come back.  An RFC3164 context fixes the year of year-less timestamps at the start of each
+/// call; an LTSV context's "Missing value" lines are printed to stdout before their record is sent or reported.
 pub struct FusedGelfLineSplitter {
     pub gpu: CudaDecoder,
     pub extra: Vec<(String, String)>,   // output.gelf_extra (gelf_encoder.rs:29-48)
@@ -582,10 +602,13 @@ impl<T: Read> Splitter<T> for FusedGelfLineSplitter {
         let max_bytes = self.max_bytes.min(self.gpu.capacity_bytes());
         run_blocks(buf_reader, max_bytes, |block| {
             decode_fitting(&self.gpu, block, &mut |gpu: &CudaDecoder, part: &[u8]| {
-                gpu.split_decode_encode_gelf(part, &self.extra, |line, r| match r {
-                    Ok(json) => tx.send(json.to_vec()).unwrap(),
-                    Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
-                    Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
+                gpu.split_decode_encode_gelf(part, &self.extra, |line, r, side| {
+                    for s in side { println!("{}", s); }  // ltsv_decoder.rs:99
+                    match r {
+                        Ok(json) => tx.send(json.to_vec()).unwrap(),
+                        Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
+                        Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
+                    }
                 })
             })
         });

@@ -1,14 +1,14 @@
 """Framing on the device vs on the host for the fused GELF pipelines (output.format = "gelf", input.format = "rfc5424",
-the default pair, or "rfc3164").
+the default pair, "rfc3164" or "ltsv").
 
-    python tools/bench_split_encode.py [--format rfc5424|rfc3164] [--lines 10000000] [--steps 10] [--warmup 2]
-                                       [--splitter-gb 1.0] [--splitter-only]
+    python tools/bench_split_encode.py [--format rfc5424|rfc3164|ltsv] [--ltsv-typed] [--lines 10000000] [--steps 10]
+                                       [--warmup 2] [--splitter-gb 1.0] [--splitter-only]
 
-On the workload of bench.py for the format (rfc5424: C2, seed 5424; rfc3164: seed 3164, year 2026; the same mean line
-length), joined with '\\n' in pinned memory:
+On the workload of bench.py for the format (rfc5424: C2, seed 5424; rfc3164: seed 3164, year 2026; ltsv: seed 1757,
+with --ltsv-typed bench.py's schema and suffixes; the same mean line length), joined with '\\n' in pinned memory:
   1. fg_split_decode_encode_gelf on the raw stream and fg_decode_encode_gelf on the same lines framed beforehand (for
-     rfc3164 also fg_split_decode on the raw stream: decode only, rows + arena back), timed alternately after warm-ups;
-     the two encoding calls must return byte-identical records and statuses;
+     rfc3164 and ltsv also fg_split_decode on the raw stream: decode only, rows + side tables back), timed alternately
+     after warm-ups; the two encoding calls must return byte-identical records, statuses and (ltsv) "Missing value" stops;
   2. the C++ BatchingLineSplitter with the fused GELF encoder end to end over at least --splitter-gb of the same text
      (text in, every JSON record handed to the sender, stderr captured).
 Prints one JSON line per section, with the card's name and power limit.  --splitter-only runs section 2 alone."""
@@ -26,10 +26,12 @@ import numpy as np
 REPO = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(REPO))
 
+import bench  # noqa: E402
 import flowgger_b200 as fb  # noqa: E402
 
 # bench.py: SEEDS, GEN_MEAN and RFC3164_YEAR (the year of a timestamp without one, fixed so that a run is reproducible)
-WORKLOADS = {"rfc5424": (fb.FMT_RFC5424, 5424, 169.2), "rfc3164": (fb.FMT_RFC3164, 3164, 140.0)}
+WORKLOADS = {"rfc5424": (fb.FMT_RFC5424, 5424, 169.2), "rfc3164": (fb.FMT_RFC3164, 3164, 140.0),
+             "ltsv": (fb.FMT_LTSV, bench.SEEDS["ltsv"], bench.GEN_MEAN["ltsv"])}
 RFC3164_YEAR = 2026
 
 
@@ -49,8 +51,10 @@ def workload(fmt_name: str, n: int) -> tuple[np.ndarray, np.ndarray]:
     return fb.generate(fmt, seed, n, mean_len=mean, bad_frac=0.005, nthreads=32, terminated=True)
 
 
-def decoder(fmt_name: str, **kw) -> fb.BatchDecoder:
+def decoder(fmt_name: str, typed: bool = False, **kw) -> fb.BatchDecoder:
     fmt = WORKLOADS[fmt_name][0]
+    if fmt == fb.FMT_LTSV and typed:
+        kw.update(ltsv_schema=bench.LTSV_SCHEMA, ltsv_suffixes=bench.LTSV_SUFFIXES)
     return fb.BatchDecoder(fmt, rfc3164_year=RFC3164_YEAR if fmt == fb.FMT_RFC3164 else 0, **kw)
 
 
@@ -61,8 +65,8 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
     loffs = (soffs - np.arange(n + 1, dtype=np.int64)).astype(np.int32)
     del keep
     cap = dict(max_batch_bytes=len(stream) + (1 << 20), max_batch_lines=n + 64)
-    split, pre = decoder(args.format, **cap), decoder(args.format, **cap)
-    decode = decoder(args.format, **cap) if args.format == "rfc3164" else None
+    split, pre = decoder(args.format, args.ltsv_typed, **cap), decoder(args.format, args.ltsv_typed, **cap)
+    decode = decoder(args.format, args.ltsv_typed, **cap) if args.format != "rfc5424" else None
     try:
         hs = split.host_alloc(len(stream))
         hs[:] = stream
@@ -103,11 +107,13 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
         assert len(ss) == n and np.array_equal(sl, soffs), "the device framed other lines than the generator made"
         assert np.array_equal(so, po) and np.array_equal(ss, ps) and np.array_equal(sb, pb), \
             "fg_split_decode_encode_gelf and fg_decode_encode_gelf disagree"
+        if args.format == "ltsv":
+            assert np.array_equal(split.ltsv_stops(), pre.ltsv_stops()), "the two calls disagree on the Missing value stops"
         out_bytes = int(so[-1])
         sections = [("split", "fg_split_decode_encode_gelf (pinned raw stream in)", len(stream)),
                     ("pre", "fg_decode_encode_gelf (pinned lines + int32 offsets in, framed beforehand)", int(loffs[-1]) + loffs.nbytes)]
         if decode is not None:
-            sections.append(("decode", "fg_split_decode (pinned raw stream in, decode only: rows + arena back, no JSON)", len(stream)))
+            sections.append(("decode", "fg_split_decode (pinned raw stream in, decode only: rows + side tables back, no JSON)", len(stream)))
         for key, api, in_bytes in sections:
             med = float(np.median(t[key]))
             rec = {"section": key, "api": api, "lines": n, "input_bytes": in_bytes, "json_bytes": out_bytes,
@@ -138,7 +144,7 @@ def splitter(args, stream: np.ndarray, info: dict) -> None:
         cuts.append(cuts[-1] + int(np.flatnonzero(stream[cuts[-1]:end] == ord("\n"))[-1]) + 1 if end < len(stream) else end)
     texts = [stream[a:b].tobytes() for a, b in zip(cuts[:-1], cuts[1:])]
     want = int(args.splitter_gb * 1e9)
-    dec = decoder(args.format, max_batch_bytes=64 << 20, max_batch_lines=1 << 20)
+    dec = decoder(args.format, args.ltsv_typed, max_batch_bytes=64 << 20, max_batch_lines=1 << 20)
     wall, in_bytes, json_bytes, lines, n_rec, n_err = 0.0, 0, 0, 0, 0, 0
     try:
         small = texts[0][: 1 << 20]
@@ -172,10 +178,13 @@ def main() -> None:
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--splitter-gb", type=float, default=1.0)
     ap.add_argument("--splitter-only", action="store_true")
+    ap.add_argument("--ltsv-typed", action="store_true", help="ltsv: bench.py's schema and suffixes")
     args = ap.parse_args()
     info = card()
     if args.format != "rfc5424":
         info["format"] = args.format
+    if args.format == "ltsv":
+        info["ltsv_typed"] = args.ltsv_typed
     stream, soffs = workload(args.format, args.lines)
     if not args.splitter_only:
         device_paths(args, stream, soffs, info)
