@@ -14,6 +14,25 @@ typedef const uint8_t* __restrict__ bytes_t;
 
 FG_DEV bool is_digit(uint32_t c) { return (c - (uint32_t)'0') <= 9u; }
 
+// what the splitter leaves of record [lo, hi): mode 1 = BufRead::lines (line_splitter.rs:17: the '\n' goes, and one '\r'
+// before it), 2 = BufRead::split(0) (nul_splitter.rs:18: only the NUL goes), 0 = the caller framed the record; returns
+// the new hi.  A record that is not UTF-8 is reported and skipped (:22-25): that flag is the call site's to look up.
+FG_DEV int strip_terminator(bytes_t p, int lo, int hi, int mode) {
+    if (mode == 0 || hi <= lo) return hi;
+    if (mode == 2) return p[hi - 1] == 0 ? hi - 1 : hi;
+    if (p[hi - 1] == '\n') {
+        --hi;
+        if (hi > lo && p[hi - 1] == '\r') --hi;
+    }
+    return hi;
+}
+
+// A CTA stages the byte span of its lines with one bulk copy of 16-byte granules (fg_tma.cuh): the span starts at the
+// granule that holds the first line's first byte and is copied up to the end of the granule that holds its last byte
+// (<= tile_bytes, a multiple of 512, when the lines fit; the input buffer is padded).
+FG_DEV int span_base(int first_offset) { return first_offset & ~15; }
+FG_DEV uint32_t span_copy_bytes(int base, int oend) { return (uint32_t)((oend - base) + 15) & ~15u; }
+
 // ---------------------------------------------------------------------------
 // str::trim / trim_end — Unicode White_Space, matched byte-wise on valid UTF-8
 // (rfc5424_decoder.rs:46,167).  U+0009-000D, 0020, 0085, 00A0, 1680,

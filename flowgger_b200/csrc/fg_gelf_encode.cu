@@ -731,19 +731,13 @@ struct EncShared {
 };
 
 __device__ __forceinline__ ByteSource stage_lines(const GelfEncodeParams& P, uint8_t* tile, uint64_t* mbar, int first, int last) {
-    const int o_first = P.offsets[first], o_last = P.offsets[last];
-    const int base = o_first & ~15;
-    const uint32_t nbytes = (uint32_t)((o_last - base) + 15) & ~15u;
-    const bool staged = nbytes <= (uint32_t)P.tile_bytes;  // CTA-uniform
-    if (staged) {
-        if (threadIdx.x == 0) {
-            mbar_init(mbar, 1);
-            fence_proxy_async();
-            mbar_expect_tx(mbar, nbytes);
-            bulk_g2s(tile, P.bytes + base, nbytes, mbar);
-        }
-        __syncthreads();  // the barrier is initialised before anyone waits on it
-        mbar_wait(mbar, 0);
+    TileStage stage = {mbar};
+    stage.init();
+    const int base = span_base(P.offsets[first]);
+    const uint32_t nbytes = span_copy_bytes(base, P.offsets[last]);
+    if (nbytes <= (uint32_t)P.tile_bytes) {  // CTA-uniform
+        __syncthreads();                     // the barrier is initialised before anyone arrives or waits on it
+        stage.load(tile, P.bytes + base, nbytes);
         return ByteSource{tile, base};
     }
     return ByteSource{P.bytes, 0};

@@ -33,37 +33,18 @@ __global__ void __launch_bounds__(kLines, kR3164CtasPerSm) parse3164_kernel(cons
     const int first = blockIdx.x * kLines;
     const int last = min(P.n, first + kLines);
     const int i = first + tid;
-    if (tid == 0) mbar_init(&mbar, 1);
-    int o0 = 0, o1 = 0;
-    if (i < last) {
-        o0 = __ldg(P.offsets + i);
-        o1 = __ldg(P.offsets + i + 1);
-    }
-    const int base = __ldg(P.offsets + first) & ~15;
-    const bool fits = i < last && o1 - base <= P.tile_bytes;  // offsets are monotone: a prefix of the CTA's lines
-    const int r = __syncthreads_count(fits);                  // (also publishes the mbarrier initialisation)
-    if (r > 0) {
-        if (tid == 0) {
-            const int oend = __ldg(P.offsets + first + r);
-            const uint32_t nbytes = (uint32_t)((oend - base) + 15) & ~15u;  // <= tile_bytes (a multiple of 512); the input buffer is padded
-            mbar_expect_tx(&mbar, nbytes);
-            bulk_g2s(tile, P.bytes + base, nbytes, &mbar);
-        }
-        mbar_wait(&mbar, 0u);
-    }
+    TileStage tstage = {&mbar};
+    tstage.init();
     const bool have = i < last;
+    const TileRound t = plan_round(P.offsets, first, last, P.tile_bytes, have);  // (its barrier also publishes the mbarrier initialisation)
+    const int o0 = t.o0, o1 = t.o1, base = t.base;
+    const bool fits = tid < t.r;  // one round: the lines behind this prefix are read from global memory
+    if (t.r > 0) tstage.load(tile, P.bytes + base, span_copy_bytes(base, __ldg(P.offsets + first + t.r)));
     const uint8_t* lp = fits ? tile + (o0 - base) : P.bytes + o0;
     int len = o1 - o0;
     bool bad_utf8 = false;
     if (have && P.strip_eol && len > 0) {
-        // BufRead::lines drops the '\n' and one '\r' before it (line_splitter.rs:17); BufRead::split(0) only the NUL
-        // (nul_splitter.rs:18); a record that is not UTF-8 is reported and skipped (:22-25)
-        if (P.strip_eol == 2) {
-            if (lp[len - 1] == 0) --len;
-        } else if (lp[len - 1] == '\n') {
-            --len;
-            if (len > 0 && lp[len - 1] == '\r') --len;
-        }
+        len = strip_terminator(lp, 0, len, P.strip_eol);
         bad_utf8 = P.line_invalid != nullptr && P.line_invalid[i] != 0;
     }
     R3Out res;

@@ -43,34 +43,23 @@ __global__ void __launch_bounds__(LINES, MINB) parse5424_kernel(const __grid_con
     // the bitmap I ("may end a token") lives behind the tile: tile_bytes / 8 + 16 bytes
     uint32_t* bmI = reinterpret_cast<uint32_t*>(tile + P.tile_bytes);
     if (*P.bad_offsets) return;  // CTA-uniform
-    if (tid == 0) mbar_init(&mbar, 1);
+    TileStage tstage = {&mbar};
+    tstage.init();
     __syncthreads();
 
-    uint32_t parity = 0;
     int cur = first;
     while (cur < last) {
         const int i = cur + tid;
-        const int o0 = __ldg(P.offsets + min(i, last));
-        const int o1 = __ldg(P.offsets + min(i + 1, last));
-        const int ocur = __ldg(P.offsets + cur);
-        const int base = ocur & ~15;
-        const bool fits = (i < last) && (o1 - base <= P.tile_bytes);
-        const int r = __syncthreads_count(fits);  // offsets are monotone: `fits` is a prefix property
+        const TileRound t = plan_round(P.offsets, cur, last, P.tile_bytes, true);
+        const int o0 = t.o0, o1 = t.o1, base = t.base, r = t.r;
         if (r == 0) {
             // the first pending line alone exceeds the tile: the wide kernel takes it
             if (tid == 0) P.wide_list[atomicAdd(P.counters + K5_WIDE_LIST, 1u)] = (uint32_t)cur;
             cur += 1;
             continue;
         }
-        const int oend = __ldg(P.offsets + cur + r);
-        const uint32_t nbytes = (uint32_t)((oend - base) + 15) & ~15u;
-        if (tid == 0) {
-            fence_proxy_async();  // generic-proxy accesses of the previous round happen-before this async write
-            mbar_expect_tx(&mbar, nbytes);
-            bulk_g2s(tile, P.bytes + base, nbytes, &mbar);
-        }
-        mbar_wait(&mbar, parity);
-        parity ^= 1u;
+        const uint32_t nbytes = span_copy_bytes(base, __ldg(P.offsets + cur + r));
+        tstage.load(tile, P.bytes + base, nbytes);
 
         // ---- stage 1: structural bitmap of the whole tile, 32 bytes (= one bitmap word) per thread per step -------
         const int nword = (int)((nbytes + 31u) >> 5);  // the tile allocation is a multiple of 512 bytes: reading the odd granule is safe
@@ -89,13 +78,7 @@ __global__ void __launch_bounds__(LINES, MINB) parse5424_kernel(const __grid_con
         int le = active ? o1 - base : 0;
         bool bad_utf8 = false;
         if (P.strip_eol && le > ls) {
-            // BufRead::lines: drop the '\n' and one '\r' before it (line_splitter.rs:17); invalid UTF-8 lines are skipped (:22-25)
-            if (P.strip_eol == 2) {  // BufRead::split(0): only the NUL terminator goes (nul_splitter.rs:18)
-                if (tile[le - 1] == 0) --le;
-            } else if (tile[le - 1] == '\n') {
-                --le;
-                if (le > ls && tile[le - 1] == '\r') --le;
-            }
+            le = strip_terminator(tile, ls, le, P.strip_eol);
             if (P.line_invalid != nullptr && P.line_invalid[i]) bad_utf8 = true;
         }
         const bool too_long = le - ls > 65535;
@@ -267,12 +250,7 @@ __device__ __forceinline__ void wide_lines(const Parse5424Params& P, int (*marks
             o0 = P.offsets[line];
             len = P.offsets[line + 1] - o0;
             if (P.strip_eol && len > 0) {
-                if (P.strip_eol == 2) {
-                    if (P.bytes[o0 + len - 1] == 0) --len;
-                } else if (P.bytes[o0 + len - 1] == '\n') {
-                    --len;
-                    if (len > 0 && P.bytes[o0 + len - 1] == '\r') --len;
-                }
+                len = strip_terminator(P.bytes, o0, o0 + len, P.strip_eol) - o0;
                 if (P.line_invalid != nullptr && P.line_invalid[line]) bad_utf8 = true;
             }
             if (bad_utf8) len = 0;

@@ -73,40 +73,27 @@ __global__ void __launch_bounds__(kThreads, kGelfCtasPerSm) parse_gelf_kernel(co
     uint8_t* slot_line = st_meta + kSlots;
     const uint32_t lane = (uint32_t)tid & 31u, wid = (uint32_t)tid >> 5;
     if (*P.bad_offsets) return;  // CTA-uniform
-    if (tid == 0) mbar_init(&mbar, 1);
+    TileStage tstage = {&mbar};
+    tstage.init();
     __syncthreads();
 
     const EntrySink sink = {P.entry_name, P.entry_val, P.entry_meta};
     const EntrySink stage = {st_name, st_val, st_meta};
-    uint32_t parity = 0;
     int cur = first;
     while (cur < last) {
         const bool lt = tid < kLines;  // line threads
         const int i = cur + tid;
-        int o0 = 0, o1 = 0;
-        if (lt) {
-            o0 = __ldg(P.offsets + min(i, last));
-            o1 = __ldg(P.offsets + min(i + 1, last));
-        }
-        const int ocur = __ldg(P.offsets + cur);
-        const int base = ocur & ~15;
-        const bool fits = lt && (i < last) && (o1 - base <= P.tile_bytes);
-        int r = __syncthreads_count(fits);  // offsets are monotone: `fits` is a prefix property
+        const TileRound t = plan_round(P.offsets, cur, last, P.tile_bytes, lt);
+        const int o0 = t.o0, o1 = t.o1, base = t.base;
+        int r = t.r;
         if (r == 0) {
             // the first pending line alone exceeds the tile: the slow kernel takes it
             if (tid == 0) P.slow_list[atomicAdd(P.slow_count, 1u)] = (uint32_t)cur;
             cur += 1;
             continue;
         }
-        const int oend = __ldg(P.offsets + cur + r);
-        const uint32_t nbytes = (uint32_t)((oend - base) + 15) & ~15u;
-        if (tid == 0) {
-            fence_proxy_async();  // generic-proxy accesses of the previous round happen-before this async write
-            mbar_expect_tx(&mbar, nbytes);
-            bulk_g2s(tile, P.bytes + base, nbytes, &mbar);
-        }
-        mbar_wait(&mbar, parity);
-        parity ^= 1u;
+        const uint32_t nbytes = span_copy_bytes(base, __ldg(P.offsets + cur + r));
+        tstage.load(tile, P.bytes + base, nbytes);
 
         // ---- (2) the three bitmaps of the whole tile, 32 bytes (= one word of each) per thread per step ----------------------
         const int nword = (int)((nbytes + 31u) >> 5);
@@ -137,13 +124,7 @@ __global__ void __launch_bounds__(kThreads, kGelfCtasPerSm) parse_gelf_kernel(co
         int le = active ? o1 - base : 0;
         bool bad_utf8 = false;
         if (active && P.strip_eol && le > ls) {
-            // BufRead::lines: drop the '\n' and one '\r' before it (line_splitter.rs:17); invalid UTF-8 lines are skipped (:22-25)
-            if (P.strip_eol == 2) {  // BufRead::split(0): only the NUL terminator goes (nul_splitter.rs:18)
-                if (tile[le - 1] == 0) --le;
-            } else if (tile[le - 1] == '\n') {
-                --le;
-                if (le > ls && tile[le - 1] == '\r') --le;
-            }
+            le = strip_terminator(tile, ls, le, P.strip_eol);
             if (P.line_invalid != nullptr && P.line_invalid[i]) bad_utf8 = true;
         }
         const bool walk = active && !bad_utf8;
@@ -314,14 +295,7 @@ __global__ void __launch_bounds__(128) post_gelf_kernel(const __grid_constant__ 
             line = (int)P.slow_list[j];
             o0 = P.offsets[line];
             len = P.offsets[line + 1] - o0;
-            if (P.strip_eol && len > 0) {
-                if (P.strip_eol == 2) {
-                    if (P.bytes[o0 + len - 1] == 0) --len;
-                } else if (P.bytes[o0 + len - 1] == '\n') {
-                    --len;
-                    if (len > 0 && P.bytes[o0 + len - 1] == '\r') --len;
-                }
-            }
+            len = strip_terminator(P.bytes, o0, o0 + len, P.strip_eol) - o0;
         }
         LineResult res;
         const uint32_t sidx = (uint32_t)o0 / 3u;  // a top-level member needs >= 5 input bytes (`"":0,`)

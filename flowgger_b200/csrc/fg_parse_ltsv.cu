@@ -51,13 +51,7 @@ __device__ __forceinline__ void direct_line(const ParseParams& P, int line, cons
     int len = act ? __ldg(P.offsets + line + 1) - d0 : 0;
     bool bad_utf8 = false;
     if (act && P.strip_eol && len > 0) {
-        const uint8_t* lp = P.bytes + d0;
-        if (P.strip_eol == 2) {
-            if (lp[len - 1] == 0) --len;
-        } else if (lp[len - 1] == '\n') {
-            --len;
-            if (len > 0 && lp[len - 1] == '\r') --len;
-        }
+        len = strip_terminator(P.bytes + d0, 0, len, P.strip_eol);
         if (P.line_invalid != nullptr && P.line_invalid[line]) {
             bad_utf8 = true;
             len = 0;
@@ -136,7 +130,8 @@ __global__ void __launch_bounds__(kThreads, kLtsvCtasPerSm) parse_ltsv_kernel(co
     uint16_t* ylist = tabs + kStageSlots;  // TYPED only: the typed rows' slots, grouped by type
     uint8_t* slot_line = reinterpret_cast<uint8_t*>(ylist + (TYPED ? kStageSlots : 0));
     if (*P.bad_offsets) return;  // CTA-uniform
-    if (tid == 0) mbar_init(&mbar, 1);
+    TileStage tstage = {&mbar};
+    tstage.init();
     LtsvDeviceConfig cfg = P.ltsv;
     LtsvSchemaView S = {cfg.names, cfg.name_off, cfg.types, cfg.n_schema, 0xFFFFFFFFu, nullptr};
     if (TYPED) {
@@ -161,23 +156,17 @@ __global__ void __launch_bounds__(kThreads, kLtsvCtasPerSm) parse_ltsv_kernel(co
 
     const EntrySink sink = {P.entry_name, P.entry_val, P.entry_meta};
     const EntrySink tmp = {P.tmp_name, P.tmp_val, P.tmp_meta};
-    uint32_t parity = 0;
     int cur = first;
     bool direct_next = false;  // CTA-uniform: line `cur` must take the direct path (more parts than the CTA has slots)
     while (cur < last) {
         // ---- the lines of this round ------------------------------------------------------------------------------
         const bool lt = tid < kLines;  // line threads
         const int i = cur + tid;
-        int o0 = 0, o1 = 0;
-        if (lt) {
-            o0 = __ldg(P.offsets + min(i, last));
-            o1 = __ldg(P.offsets + min(i + 1, last));
-        }
-        const int ocur = __ldg(P.offsets + cur);
-        const int base = ocur & ~15;
         // tile_bytes <= 65024 (launch_parse_ltsv): a line inside the tile is shorter than 64 KiB, positions fit 16 bits
-        const bool fits = lt && !direct_next && (i < last) && (o1 - base <= P.tile_bytes);
-        int r = __syncthreads_count(fits);  // offsets are monotone: `fits` is a prefix property
+        // (a direct_next round has no tile — no line fits -1 bytes — so r == 0 sends line `cur` down the direct path)
+        const TileRound t = plan_round(P.offsets, cur, last, direct_next ? -1 : P.tile_bytes, lt);
+        const int o0 = t.o0, o1 = t.o1, base = t.base;
+        int r = t.r;
         if (r == 0) {
             direct_next = false;
             direct_line(P, cur, sink, tmp);
@@ -185,15 +174,8 @@ __global__ void __launch_bounds__(kThreads, kLtsvCtasPerSm) parse_ltsv_kernel(co
             cur += 1;
             continue;
         }
-        const int oend = __ldg(P.offsets + cur + r);
-        const uint32_t nbytes = (uint32_t)((oend - base) + 15) & ~15u;
-        if (tid == 0) {
-            fence_proxy_async();  // generic-proxy accesses of the previous round happen-before this async write
-            mbar_expect_tx(&mbar, nbytes);
-            bulk_g2s(tile, P.bytes + base, nbytes, &mbar);
-        }
-        mbar_wait(&mbar, parity);
-        parity ^= 1u;
+        const uint32_t nbytes = span_copy_bytes(base, __ldg(P.offsets + cur + r));
+        tstage.load(tile, P.bytes + base, nbytes);
 
         // ---- (2) the TAB bitmap of the whole tile, 32 bytes (= one word) per thread per step --------------------------
         const int nword = (int)((nbytes + 31u) >> 5);  // the tile allocation is a multiple of 512 bytes: reading the odd granule is safe
@@ -209,13 +191,7 @@ __global__ void __launch_bounds__(kThreads, kLtsvCtasPerSm) parse_ltsv_kernel(co
         int le = active ? o1 - base : 0;
         bool bad_utf8 = false;
         if (active && P.strip_eol && le > ls) {
-            // BufRead::lines: drop the '\n' and one '\r' before it (line_splitter.rs:17); invalid UTF-8 lines are skipped (:22-25)
-            if (P.strip_eol == 2) {  // BufRead::split(0): only the NUL terminator goes (nul_splitter.rs:18)
-                if (tile[le - 1] == 0) --le;
-            } else if (tile[le - 1] == '\n') {
-                --le;
-                if (le > ls && tile[le - 1] == '\r') --le;
-            }
+            le = strip_terminator(tile, ls, le, P.strip_eol);
             if (P.line_invalid != nullptr && P.line_invalid[i]) bad_utf8 = true;
         }
         const bool walk = active && !bad_utf8;

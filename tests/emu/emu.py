@@ -76,14 +76,14 @@ def classify16(block: bytes) -> int:
     return int(lib().emu5424_classify16(buf))
 
 
-def decode_dump(native, data: np.ndarray, offsets: np.ndarray, tile_bytes: int = 13312, strip_eol: bool = False,
+def decode_dump(native, data: np.ndarray, offsets: np.ndarray, tile_bytes: int = 13312, strip_eol: int = 0,
                 invalid: np.ndarray | None = None):
     """Emulated RFC5424 decode -> (canonical dumps, dump offsets, FgBatchOut fields as a dict) through the product's
     host materialiser (fgh_dump_records)."""
     from flowgger_b200.native import FgBatchOut, dump_records
     out = FgBatchOut()
     n = len(offsets) - 1
-    lib().emu5424_decode(C.c_void_p(data.ctypes.data), C.c_void_p(offsets.ctypes.data), n, tile_bytes, 1 if strip_eol else 0,
+    lib().emu5424_decode(C.c_void_p(data.ctypes.data), C.c_void_p(offsets.ctypes.data), n, tile_bytes, int(strip_eol),
                          C.c_void_p(invalid.ctypes.data) if invalid is not None else None, C.byref(out))
     try:
         buf, offs = dump_records(native.FMT_RFC5424, out, data, offsets)

@@ -80,7 +80,7 @@ int emu_gelf_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
         const int last = std::min(n, first + kLines);
         int cur = first;
         while (cur < last) {
-            const int base = offsets[cur] & ~15;
+            const int base = fg::span_base(offsets[cur]);
             int r = 0;
             while (cur + r < last && offsets[cur + r + 1] - base <= tile_bytes) ++r;
             if (r == 0) {
@@ -89,8 +89,7 @@ int emu_gelf_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
                 continue;
             }
             ++T->rounds;
-            const int oend = offsets[cur + r];
-            const uint32_t nbytes = (uint32_t)((oend - base) + 15) & ~15u;
+            const uint32_t nbytes = fg::span_copy_bytes(base, offsets[cur + r]);
             for (uint32_t k = 0; k < nbytes; ++k) tile[k] = (int64_t)base + k < total_bytes ? bytes[base + k] : 0;  // the bulk copy
             const int nword = (int)((nbytes + 31u) >> 5);
             std::fill(anyK.begin(), anyK.end(), 0u);
@@ -112,12 +111,7 @@ int emu_gelf_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
                 int le = offsets[i + 1] - base;
                 bool bad = false;
                 if (strip_eol && le > ls) {
-                    if (strip_eol == 2) {
-                        if (tile[le - 1] == 0) --le;
-                    } else if (tile[le - 1] == '\n') {
-                        --le;
-                        if (le > ls && tile[le - 1] == '\r') --le;
-                    }
+                    le = fg::strip_terminator(tile.data(), ls, le, strip_eol);
                     if (invalid && invalid[i]) bad = true;
                 }
                 const bool walk = !bad;
@@ -187,14 +181,7 @@ int emu_gelf_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
         ++T->slow;
         const int o0 = offsets[line];
         int len = offsets[line + 1] - o0;
-        if (strip_eol && len > 0) {
-            if (strip_eol == 2) {
-                if (bytes[o0 + len - 1] == 0) --len;
-            } else if (bytes[o0 + len - 1] == '\n') {
-                --len;
-                if (len > 0 && bytes[o0 + len - 1] == '\r') --len;
-            }
-        }
+        len = fg::strip_terminator(bytes, o0, o0 + len, strip_eol) - o0;
         tname.assign((size_t)len / 3 + 64, fg_span{0, 0});
         tval.assign(tname.size(), 0);
         tmeta.assign(tname.size(), 0);

@@ -115,12 +115,7 @@ int emu_ltsv_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
         int len = offsets[i + 1] - d0;
         bool bad = false;
         if (strip_eol && len > 0) {
-            if (strip_eol == 2) {
-                if (bytes[d0 + len - 1] == 0) --len;
-            } else if (bytes[d0 + len - 1] == '\n') {
-                --len;
-                if (len > 0 && bytes[d0 + len - 1] == '\r') --len;
-            }
+            len = fg::strip_terminator(bytes + d0, 0, len, strip_eol);
             if (invalid && invalid[i]) { bad = true; len = 0; }
         }
         tname.assign((size_t)len / 2 + 2, fg_span{0, 0});
@@ -145,7 +140,7 @@ int emu_ltsv_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
         int cur = first;
         bool direct_next = false;
         while (cur < last) {
-            const int base = offsets[cur] & ~15;
+            const int base = fg::span_base(offsets[cur]);
             int r = 0;
             if (!direct_next)
                 while (cur + r < last && offsets[cur + r + 1] - base <= tile_bytes) ++r;
@@ -156,8 +151,7 @@ int emu_ltsv_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
                 continue;
             }
             ++T->rounds;
-            const int oend = offsets[cur + r];
-            const uint32_t nbytes = (uint32_t)((oend - base) + 15) & ~15u;
+            const uint32_t nbytes = fg::span_copy_bytes(base, offsets[cur + r]);
             for (uint32_t k = 0; k < nbytes; ++k) tile[k] = (int64_t)base + k < total_bytes ? bytes[base + k] : 0;  // the bulk copy
             const int nword = (int)((nbytes + 31u) >> 5);
             for (int g = 0; g < nword; ++g)
@@ -173,12 +167,7 @@ int emu_ltsv_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int
                 ls[tid] = offsets[i] - base;
                 le[tid] = offsets[i + 1] - base;
                 if (strip_eol && le[tid] > ls[tid]) {
-                    if (strip_eol == 2) {
-                        if (tile[le[tid] - 1] == 0) --le[tid];
-                    } else if (tile[le[tid] - 1] == '\n') {
-                        --le[tid];
-                        if (le[tid] > ls[tid] && tile[le[tid] - 1] == '\r') --le[tid];
-                    }
+                    le[tid] = fg::strip_terminator(tile.data(), ls[tid], le[tid], strip_eol);
                     if (invalid && invalid[i]) bad[tid] = 1;
                 }
                 nb[tid] = bad[tid] ? 0u : (uint32_t)fg::lt_count_tabs(bmT.data(), ls[tid], le[tid]) + 1u;

@@ -119,11 +119,11 @@ int emu_r3164_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, in
         cfg.arena_counter = &counter;
         for (int first = 0; first < n; first += kLines) {
             const int last = std::min(n, first + kLines);
-            const int base = offsets[first] & ~15;
+            const int base = fg::span_base(offsets[first]);
             int r = 0;
             while (first + r < last && offsets[first + r + 1] - base <= tile_bytes) ++r;
             if (r > 0) {
-                const uint32_t nbytes = (uint32_t)((offsets[first + r] - base) + 15) & ~15u;
+                const uint32_t nbytes = fg::span_copy_bytes(base, offsets[first + r]);
                 // the device buffer is padded; here only the bytes that exist are copied, the rest of the granule is zero
                 const int64_t avail = (int64_t)offsets[n] - base;
                 memset(tile0, 0, nbytes);
@@ -137,12 +137,7 @@ int emu_r3164_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, in
                 int len = o1 - o0;
                 bool bad = false;
                 if (have && strip_eol && len > 0) {
-                    if (strip_eol == 2) {
-                        if (lp[len - 1] == 0) --len;
-                    } else if (lp[len - 1] == '\n') {
-                        --len;
-                        if (len > 0 && lp[len - 1] == '\r') --len;
-                    }
+                    len = fg::strip_terminator(lp, 0, len, strip_eol);
                     bad = invalid != nullptr && invalid[i] != 0;
                 }
                 fg::R3Out res;

@@ -70,7 +70,7 @@ int emu5424_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int3
         const int last = std::min(n, first + kLines);
         int cur = first;
         while (cur < last) {
-            const int base = offsets[cur] & ~15;
+            const int base = fg::span_base(offsets[cur]);
             int r = 0;
             while (cur + r < last && offsets[cur + r + 1] - base <= tile_bytes) ++r;
             if (r == 0) {
@@ -78,8 +78,7 @@ int emu5424_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int3
                 ++cur;
                 continue;
             }
-            const int oend = offsets[cur + r];
-            const uint32_t nbytes = (uint32_t)((oend - base) + 15) & ~15u;
+            const uint32_t nbytes = fg::span_copy_bytes(base, offsets[cur + r]);
             for (uint32_t k = 0; k < nbytes; ++k) tile[k] = (int64_t)base + k < total_bytes ? bytes[base + k] : 0;  // the bulk copy
             uint16_t* bmI16 = (uint16_t*)bmI.data();
             const int ngran = (int)(nbytes >> 4);
@@ -91,10 +90,7 @@ int emu5424_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int3
                 int le = offsets[i + 1] - base;
                 bool bad = false;
                 if (strip_eol && le > ls) {
-                    if (tile[le - 1] == '\n') {
-                        --le;
-                        if (le > ls && tile[le - 1] == '\r') --le;
-                    }
+                    le = fg::strip_terminator(tile.data(), ls, le, strip_eol);
                     if (invalid && invalid[i]) bad = true;
                 }
                 const bool too_long = le - ls > 65535;
@@ -117,7 +113,7 @@ int emu5424_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int3
             cur += r;
         }
     }
-    // unescape5424_kernel: arena records are [u16 length][bytes], 2-byte aligned
+    // post5424_kernel, unescape_lines: arena records are [u16 length][bytes], 2-byte aligned
     for (uint32_t line : T->esc_list) {
         const fg_row5424& row = T->rows[line];
         const int o0 = offsets[line];
@@ -133,16 +129,13 @@ int emu5424_decode(const uint8_t* bytes, const int32_t* offsets, int32_t n, int3
             }
         }
     }
-    // wide5424_kernel
+    // post5424_kernel, wide_lines
     for (uint32_t line : T->wide_list) {
         const int o0 = offsets[line];
         int len = offsets[line + 1] - o0;
         bool bad = false;
         if (strip_eol && len > 0) {
-            if (bytes[o0 + len - 1] == '\n') {
-                --len;
-                if (len > 0 && bytes[o0 + len - 1] == '\r') --len;
-            }
+            len = fg::strip_terminator(bytes, o0, o0 + len, strip_eol) - o0;
             if (invalid && invalid[line]) bad = true;
         }
         if (bad) len = 0;

@@ -107,10 +107,15 @@ def test_mutation_fuzz(emu, native, oracle):
 
 def test_split_mode_terminators(emu, native, oracle):
     lines = [V.G1_LINE.encode(), V.G2_LINE.encode(), b"", b"abc"]
-    raw = [l + (b"\r\n" if k % 2 else b"\n") for k, l in enumerate(lines)]
-    data, offs = oracle.pack(raw)
-    gbuf, goffs, _ = emu.decode_dump(native, data, offs, strip_eol=True)
     d0, o0 = oracle.pack(lines)
     obuf, ooffs = oracle.decode_dump(R5, d0, o0, None)
-    # spans differ by construction (terminators inside the stream); the decoded Records must not
-    assert [gbuf[goffs[i]:goffs[i + 1]] for i in range(len(lines))] == [obuf[ooffs[i]:ooffs[i + 1]] for i in range(len(lines))]
+    want = [obuf[ooffs[i]:ooffs[i + 1]] for i in range(len(lines))]
+    for mode, term in ((True, [b"\n", b"\r\n"]), (2, [b"\0", b"\0"])):
+        raw = [l + term[k % 2] for k, l in enumerate(lines)]
+        data, offs = oracle.pack(raw)
+        gbuf, goffs, _ = emu.decode_dump(native, data, offs, strip_eol=mode)
+        # spans differ by construction (terminators inside the stream); the decoded Records must not
+        assert [gbuf[goffs[i]:goffs[i + 1]] for i in range(len(lines))] == want
+        inv = np.array([0, 1, 0, 0], dtype=np.uint8)
+        gbuf, goffs, _ = emu.decode_dump(native, data, offs, strip_eol=mode, invalid=inv)
+        assert gbuf[goffs[1]:goffs[2]] == b"E:Invalid UTF-8 input;out=0" and gbuf[goffs[0]:goffs[1]] == want[0]
