@@ -227,6 +227,8 @@ struct fg_ctx {
     Buf<uint8_t> enc_status;
     Buf<int32_t> enc_stop;  // LTSV: where the decoder stopped printing "Missing value" lines (fg_encoded_ltsv_stops)
     int enc_stop_n = -1;    // records of the last fused LTSV call (-1: the last fused call was not LTSV)
+    double gelf_now = 0.0;  // GELF: Record.ts of the call's records without "timestamp" (fg_encoded_gelf_now)
+    bool gelf_now_ok = false;  // the last fused call was on GELF input and succeeded
     Buf<uint8_t> scan_temp;
     size_t scan_temp_bytes = 0;
     Buf<uint8_t> static_blob;  // fixed GELF keys + output.gelf_extra, sorted
@@ -570,9 +572,19 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
 }
 
 // The decoders whose device-resident results the fused GELF encoder reads.  LTSV only on a context created for it: the
-// pair keys carry that context's ltsv_suffixes.
+// pair keys carry that context's ltsv_suffixes.  GELF likewise, the rule LTSV follows.
 bool gelf_fusable(const fg_ctx* c, int fmt) {
-    return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || (fmt == FG_FMT_LTSV && c->input_format == FG_FMT_LTSV);
+    return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || ((fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF) && c->input_format == fmt);
+}
+
+// gelf_decoder.rs:109 -> utils/mod.rs:16-21: the wall clock as secs + nanos / 1e9, read once at the start of a fused GELF
+// call for all its records without "timestamp"
+void begin_gelf_call(fg_ctx* c, int fmt) {
+    c->gelf_now_ok = false;
+    if (fmt != FG_FMT_GELF) return;
+    timespec t;
+    clock_gettime(CLOCK_REALTIME, &t);
+    c->gelf_now = (double)t.tv_sec + (double)t.tv_nsec / 1e9;
 }
 
 // The fused GELF encoder over the decoder's results of lines [l0, l0 + n), parse step k
@@ -591,8 +603,12 @@ int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream
         E.col_msg = (const int2*)(r + col_off(c, C_MSG)) + l0;
         E.col_full = (const int2*)(r + col_off(c, C_FULL)) + l0;
     }
+    if (fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF) E.col_sd = (const int2*)(c->rows.d + col_off(c, C_SD)) + l0;
+    if (fmt == FG_FMT_GELF) {
+        E.gelf_now = c->gelf_now;
+        E.gelf_entries = c->k.d + fg::K5_ENTRIES;
+    }
     if (fmt == FG_FMT_LTSV) {
-        E.col_sd = (const int2*)(c->rows.d + col_off(c, C_SD)) + l0;
         E.ltsv_suffix = c->ltsv.suffix;
         for (int t = 0; t < 6; ++t) E.ltsv_suffix_off[t] = c->ltsv.suffix_off[t];
         E.ltsv_stop = c->enc_stop.d + l0;
@@ -1192,12 +1208,13 @@ int fg_set_gelf_extra(fg_ctx* c, int32_t n, const char* const* keys, const char*
     return build_static_items(c);
 }
 
-// decode (RFC5424, RFC3164 or LTSV) + GelfEncoder::encode fused: H2D lines -> parse kernels -> size / scan / write
+// decode (RFC5424, RFC3164, LTSV or GELF) + GelfEncoder::encode fused: H2D lines -> parse kernels -> size / scan / write
 // kernels -> D2H of the encoded records (and for LTSV the "Missing value" stops) only, chunk by chunk; the decoder's rows
 // and side tables never leave the device.
 int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
     if (!c || !out) return FG_E_ARG;
     c->enc_stop_n = -1;  // the stops of an earlier call end here, whatever this one returns
+    begin_gelf_call(c, (int)fmt);
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
     if (!gelf_fusable(c, (int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
     if (int rc = begin_call(c, fmt)) return rc;
@@ -1211,6 +1228,7 @@ int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const 
     if (n == 0) {
         c->enc_offsets.h[0] = 0;
         if (fmt == FG_FMT_LTSV) c->enc_stop_n = 0;
+        c->gelf_now_ok = fmt == FG_FMT_GELF;
         return FG_OK;
     }
     const auto t_begin = std::chrono::steady_clock::now();
@@ -1243,6 +1261,7 @@ int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const 
         out->kernel_ms = kms;
         out->total_ms = tms;
         if (fmt == FG_FMT_LTSV) c->enc_stop_n = n;
+        c->gelf_now_ok = fmt == FG_FMT_GELF;
         return FG_OK;
     }
     return fail(c, FG_E_CAPACITY, "output / side table overflow after regrow");
@@ -1251,6 +1270,12 @@ int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const 
 int fg_encoded_ltsv_stops(const fg_ctx* c, const int32_t** stop) {
     if (!c || !stop || c->enc_stop_n < 0) return FG_E_ARG;
     *stop = c->enc_stop.h;
+    return FG_OK;
+}
+
+int fg_encoded_gelf_now(const fg_ctx* c, double* now) {
+    if (!c || !now || !c->gelf_now_ok) return FG_E_ARG;
+    *now = c->gelf_now;
     return FG_OK;
 }
 
@@ -1398,18 +1423,20 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
     return FG_OK;
 }
 
-// framing + decode (RFC5424, RFC3164 or LTSV) + GelfEncoder::encode on the device: only the encoded records, the line
+// framing + decode (RFC5424, RFC3164, LTSV or GELF) + GelfEncoder::encode on the device: only the encoded records, the line
 // offsets and for LTSV the "Missing value" stops come back
 int fg_split_decode_encode_gelf(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
                                 const int32_t** line_offsets) {
     if (!c || !out || !line_offsets) return FG_E_ARG;
     c->enc_stop_n = -1;  // the stops of an earlier call end here, whatever this one returns
+    begin_gelf_call(c, (int)fmt);
     if (!gelf_fusable(c, (int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
     int32_t n;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;
     if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, true, n, total, kms, tms)) return rc;
     if (fmt == FG_FMT_LTSV) c->enc_stop_n = n;
+    c->gelf_now_ok = fmt == FG_FMT_GELF;
     memset(out, 0, sizeof *out);
     out->n = n;
     out->bytes = c->enc_out.h;

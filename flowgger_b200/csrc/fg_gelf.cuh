@@ -324,6 +324,34 @@ static __device__ __noinline__ bool json_str_is(bytes_t p, int a0, int a1, bool 
     return key_iter_next(x) < 0;
 }
 
+// serde_json 0.8 ser.rs escape_bytes: `"` `\` \b \f \n \r \t get a backslash form (returns the second byte), else 0
+FG_DEV uint32_t json_escape_of(uint32_t c) {
+    if (c == '"' || c == '\\') return c;
+    if (c >= 0x20u) return 0u;
+    return c == 8u ? 'b' : c == 9u ? 't' : c == 10u ? 'n' : c == 12u ? 'f' : c == 13u ? 'r' : 0u;
+}
+
+// One step of re-encoding a validated JSON string body p[i, end) as the text serde_json prints for its unescaped bytes
+// (GelfDecoder::decode unescapes, GelfEncoder::encode escapes again): the source escape — or raw byte — at p[i] becomes
+// 1..4 output bytes in w (low byte first), i moves past it; returns the byte count.  The unescape is KeyIter's and the
+// escape json_escape_of, so decoder and encoder cannot disagree on what a string holds.  At most 4 bytes: a \uXXXX
+// gives 1..3 bytes of UTF-8 (a byte below 0x80 escaped to 2 at most), a surrogate pair 4, `\` + LF of a retry line
+// the 3 bytes `\\n`.
+FG_DEV int json_transcode_step(bytes_t p, int& i, int end, bool mode2, uint32_t& w) {
+    KeyIter it;
+    key_iter_init(it, p, i, end, mode2);
+    w = 0;
+    int n = 0;
+    do {
+        const uint32_t c = (uint32_t)key_iter_next(it);
+        const uint32_t e = json_escape_of(c);
+        w |= (e ? ('\\' | (e << 8)) : c) << (8 * n);
+        n += e ? 2 : 1;
+    } while (it.npend);
+    i = it.i;
+    return n;
+}
+
 
 // Top-level members of one line while it is being parsed: the first kMaxLocalMembers live in per-thread local
 // memory (L1-resident); an object with more members spills everything to the scratch table (rare).

@@ -6,7 +6,7 @@
 // an earlier one (SD pairs replace fixed fields, output.gelf_extra replaces everything), compact separators, strings
 // with `"` `\\` \b \f \n \r \t escaped, Record.ts through dtoa (fg_dtoa.cuh).
 //
-// Input = the decoder's device-resident results; nothing of them travels to the host in this mode.  Three record
+// Input = the decoder's device-resident results; nothing of them travels to the host in this mode.  Four record
 // sources, chosen at compile time (the kernels are templates on the source, everything after the record view is shared):
 //   From5424  compact rows + 8-byte entries + arena, or wide rows (structured data; every fixed field present)
 //   From3164  the row columns of parse3164_kernel + the arena of re-joined messages (rfc3164_decoder.rs:71-82, 106-117:
@@ -15,6 +15,11 @@
 //             or sd_id; no severity without `level`; msg None without `message`).  A pair's key is '_' + name + the
 //             type's suffix (FG_EM_SUFFIX), so keys are ordered and de-duplicated on that composed text; a typed value
 //             (bool, f64, i64, u64) is written as JSON, not as its source text.
+//   FromGelf  the row columns of parse_gelf_kernel / post_gelf_kernel + their 17-byte side table (gelf_decoder.rs:34-125:
+//             no appname, procid or sd_id; level, short_message and full_message only when the object has them; the
+//             wall clock of the call for a record without "timestamp").  A member's key is '_' + its name (the name alone
+//             when it starts with '_', FG_EM_NO_PREFIX); names, strings and keys are compared and written as their
+//             UNESCAPED text: a span that holds JSON escapes is re-encoded through the decoder's own KeyIter.
 // Launches per chunk of lines:
 //   gelf_size_kernel   one thread per line: exact length of its record (0 for a line the decoder rejected); the bytes of
 //                      the CTA's 256 lines are staged in shared memory by one TMA bulk copy and handed to the threads
@@ -32,6 +37,7 @@
 
 #include "fg_common.cuh"
 #include "fg_dtoa.cuh"
+#include "fg_gelf.cuh"
 #include "fg_r5fast.cuh"
 #include "fg_status.h"
 #include "fg_tma.cuh"
@@ -86,7 +92,7 @@ struct WordSink {
     }
 };
 
-// An LTSV record's sink: the extent of the side table's value column, which tells run_segments the number segments
+// An LTSV or GELF record's sink: the extent of the side table's value column, which tells the byte loop the number segments
 template <class Sink>
 struct NumSink {
     Sink& s;
@@ -126,6 +132,7 @@ struct RecView {
     bool has_sd;
     uint32_t first, count;             // entries8 range, or wide-entry range
     const uint8_t* line;
+    uint32_t flags;                    // GELF: the row's FG_FLAG_* (escaped spans, retry line)
 };
 
 // `src` = where the bytes of the caller's buffer are read from: the staged tile (src[k] = byte base + k) or global memory
@@ -314,11 +321,121 @@ __device__ __forceinline__ int cmp_sd_key(const LtsvKey& a, Span b) {
     return la == b.len - 1 ? 0 : (la < b.len - 1 ? -1 : 1);
 }
 
+// A GELF row (fg_parse_gelf.cu): the column layout of LTSV.  msg.x < 0 / full.x < 0: the object has no short_message /
+// full_message (None); a row without "timestamp" (FG_FLAG_TS_MISSING) takes the call's wall clock.
+constexpr uint32_t kTsMissing = 0x01u, kHostEsc = 0x04u, kMsgEsc = 0x08u, kFullEsc = 0x10u, kNlRetry = 0x20u;  // FG_FLAG_*
+__device__ __forceinline__ void load_view_gelf(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) {
+    const uint32_t meta = P.col_meta[i];
+    r.ok = (meta & 0xFFu) == 0u;
+    r.wide = false;
+    r.has_sd = false;
+    r.first = r.count = 0;
+    if (!r.ok) return;
+    r.severity = (meta >> 16) & 0xFFu;
+    r.flags = meta >> 24;
+    r.ts = (r.flags & kTsMissing) ? P.gelf_now : P.col_ts[i];
+    const int2 h = P.col_host[i], m = P.col_msg[i], f = P.col_full[i], sd = P.col_sd[i];
+    r.host = Span{B.at(h.x), h.y};
+    r.msg = m.x >= 0 ? Span{B.at(m.x), m.y} : Span{nullptr, 0};
+    r.full = f.x >= 0 ? Span{B.at(f.x), f.y} : Span{nullptr, 0};
+    r.first = (uint32_t)sd.x;
+    r.count = (uint32_t)sd.y;
+    // an overflowed side table (the batch is redone) leaves rows whose range names other lines' rows: read none
+    if ((unsigned long long)r.first + r.count > (unsigned long long)P.wentry_cap || *P.gelf_entries > P.wentry_cap) r.ok = false;
+}
+
+// A GELF member.  Its key after the '_' is the name, or the name without its leading '_' (FG_EM_NO_PREFIX,
+// gelf_decoder.rs:99-103); `name` is that raw span.  esc: the span holds JSON escapes (FG_EM_NAME_ESC), so its bytes are
+// read through KeyIter; plain names are compared byte by byte.  A value is a string span (tag 0; esc = FG_EM_UNESCAPE)
+// or the fg_tag of its 8 value bytes.
+struct GelfKey {
+    Span name;
+    bool esc, mode2;
+};
+struct GelfVal {
+    unsigned long long v;
+    uint32_t tag;
+    uint32_t e;  // its row
+    bool esc;
+};
+constexpr uint32_t kEmUnescape = 0x08u, kEmNoPrefix = 0x10u, kEmNameEsc = 0x40u;  // FG_EM_*
+
+__device__ __forceinline__ bool load_pair_gelf(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, uint32_t e, GelfKey& key,
+                                               GelfVal& val) {
+    const uint32_t m = P.wentry_meta[e];
+    const int2 nm = P.wentry_name[e];
+    key.name = Span{B.at(nm.x), nm.y};
+    key.esc = (m & kEmNameEsc) != 0u;
+    key.mode2 = (r.flags & kNlRetry) != 0u;
+    if (m & kEmNoPrefix) {  // drop the '_' the name starts with: one raw byte, or the escape that spells it
+        int k = 1;
+        if (key.esc) {
+            KeyIter it;
+            key_iter_init(it, key.name.p, 0, key.name.len, key.mode2);
+            key_iter_next(it);
+            k = it.i;
+        }
+        key.name.p += k;
+        key.name.len -= k;
+    }
+    val.v = P.wentry_val[e];
+    val.tag = m & 0x07u;
+    val.e = e;
+    val.esc = (m & kEmUnescape) != 0u;
+    return true;
+}
+
+// the unescaped bytes of a key, -1 at the end
+struct KeyText {
+    KeyIter it;
+    __device__ __forceinline__ explicit KeyText(const GelfKey& a) { key_iter_init(it, a.name.p, 0, a.name.len, a.mode2); }
+    __device__ __forceinline__ int next() { return key_iter_next(it); }
+};
+__device__ __forceinline__ uint32_t name_prefix(const GelfKey& n) {
+    uint32_t k = 0;
+    if (!n.esc) {
+        for (int j = 0; j < 4; ++j) k = (k << 8) | (j < n.name.len ? (uint32_t)n.name.p[j] : 0u);
+        return k;
+    }
+    KeyText t(n);
+    for (int j = 0; j < 4; ++j) {
+        const int c = t.next();
+        k = (k << 8) | (c < 0 ? 0u : (uint32_t)c);
+        if (c < 0) {
+            k <<= 8 * (3 - j);
+            break;
+        }
+    }
+    return k;
+}
+__device__ __forceinline__ int cmp_names(const GelfKey& a, const GelfKey& b) {
+    if (!a.esc && !b.esc) return cmp_names(a.name, b.name);
+    KeyText x(a), y(b);
+    for (;;) {
+        const int cx = x.next(), cy = y.next();
+        if (cx != cy) return cx < cy ? -1 : 1;
+        if (cx < 0) return 0;
+    }
+}
+// byte-order comparison of ('_' + key) with b
+__device__ __forceinline__ int cmp_sd_key(const GelfKey& a, Span b) {
+    if (!a.esc) return cmp_sd_key(a.name, b);
+    if (b.len == 0) return 1;
+    if ((uint32_t)'_' != b.p[0]) return (uint32_t)'_' < b.p[0] ? -1 : 1;
+    KeyText x(a);
+    for (int k = 1;; ++k) {
+        const int cx = x.next(), cy = k < b.len ? (int)b.p[k] : -1;
+        if (cx != cy) return cx < cy ? -1 : 1;
+        if (cx < 0) return 0;
+    }
+}
+
 // The record sources the kernels are instantiated for.  kSd: the record may carry structured data.  kOptional:
 // application_name and process_id are None, and level is None without a severity.  kLtsv: pairs are LtsvKey / LtsvVal
-// (composed keys, typed values), and the size pass writes the "Missing value" stop of every line.
+// (composed keys, typed values), and the size pass writes the "Missing value" stop of every line.  kGelf: pairs are
+// GelfKey / GelfVal, full_message may be None, and spans may hold JSON escapes.
 struct From5424 {
-    static constexpr bool kSd = true, kOptional = false, kLtsv = false;
+    static constexpr bool kSd = true, kOptional = false, kLtsv = false, kGelf = false;
     using Key = Span;
     using Val = Span;
     static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view(P, B, i, r); }
@@ -328,7 +445,7 @@ struct From5424 {
     }
 };
 struct From3164 {
-    static constexpr bool kSd = false, kOptional = true, kLtsv = false;
+    static constexpr bool kSd = false, kOptional = true, kLtsv = false, kGelf = false;
     using Key = Span;
     using Val = Span;
     static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_3164(P, B, i, r); }
@@ -338,13 +455,23 @@ struct From3164 {
     }
 };
 struct FromLtsv {
-    static constexpr bool kSd = true, kOptional = true, kLtsv = true;
+    static constexpr bool kSd = true, kOptional = true, kLtsv = true, kGelf = false;
     using Key = LtsvKey;
     using Val = LtsvVal;
     static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_ltsv(P, B, i, r); }
     static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.col_meta[i] & 0xFFu; }
     static __device__ __forceinline__ bool pair(const GelfEncodeParams& P, const ByteSource& B, const RecView&, uint32_t e, Key& k, Val& v) {
         return load_pair_ltsv(P, B, e, k, v);
+    }
+};
+struct FromGelf {
+    static constexpr bool kSd = true, kOptional = true, kLtsv = false, kGelf = true;
+    using Key = GelfKey;
+    using Val = GelfVal;
+    static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_gelf(P, B, i, r); }
+    static __device__ __forceinline__ uint32_t status(const GelfEncodeParams& P, int i) { return P.col_meta[i] & 0xFFu; }
+    static __device__ __forceinline__ bool pair(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, uint32_t e, Key& k, Val& v) {
+        return load_pair_gelf(P, B, r, e, k, v);
     }
 };
 
@@ -369,10 +496,11 @@ enum { GF_APP = 0, GF_FULL, GF_HOST, GF_LEVEL, GF_PROC, GF_SDID, GF_SHORT, GF_TS
 // produces one output byte per iteration from the current segment.
 struct Seg {
     const uint8_t* p;
-    int len;  // bit 31: JSON-escape the bytes
+    int len;  // bit 31: JSON-escape the bytes; bit 30 (GELF): the bytes are a JSON string body, re-encoded step by step
 };
 constexpr int kMaxSegs = 56;  // a record with more segments is emitted in several windows (rebuilt with `skip`)
 constexpr int kEscBit = (int)0x80000000u;
+constexpr int kJsonBit = 0x40000000;
 __device__ const uint8_t kLit[] = "{}\",\"_\":\"\"unknown\"\"-\"\"1.1\"01234567";
 //                                 0 1 2 3..5 6..8 9..17      18..20 21..25 26..33
 enum { L_OPEN = 0, L_CLOSE = 1, L_QUOTE = 2, L_PAIR = 3 /* ,"_ */, L_MID = 6 /* ":" */, L_UNKNOWN = 9, L_DASH = 18, L_V11 = 21, L_DIGITS = 26 };
@@ -401,6 +529,19 @@ struct SegList {
     // a number whose text does not exist yet (LTSV): the segment points at its 8 value bytes in the side table and holds
     // its fg_ltsv_type as length; run_segments formats it when it reaches the segment
     __device__ __forceinline__ void num(const unsigned long long* at, uint32_t tag) { push((const uint8_t*)at, (int)tag, false); }
+    // GELF: a string span as serde_json writes its unescaped text; json = the span holds JSON escapes
+    __device__ __forceinline__ void text(const uint8_t* p, int len, bool json) {
+        if (!json) {
+            push(p, len, true);
+        } else if (len > 0) {
+            push(p, len | kJsonBit, true);
+        }
+    }
+    __device__ __forceinline__ void str_json(Span v, bool json) {
+        lit(L_QUOTE, 1);
+        text(v.p, v.len, json);
+        lit(L_QUOTE, 1);
+    }
 };
 
 // `"_` is already out; the rest of an LTSV pair: `name suffix":` and its value (ltsv_decoder.rs:131-193: a typed value is
@@ -418,9 +559,29 @@ __device__ __forceinline__ void ltsv_pair(const GelfEncodeParams& P, SegList& L,
     L.num(P.wentry_val + v.e, v.tag);
 }
 
-// serde_json 0.8 for the typed values of an LTSV record: Bool as true / false, F64 through dtoa (non-finite -> null),
-// I64 / U64 in decimal
+// `"_` is already out; the rest of a GELF member: `key":` and its value (gelf_decoder.rs:91-104: the JSON value as
+// an SDValue, a string as its unescaped text)
+__device__ __forceinline__ void gelf_pair(const GelfEncodeParams& P, SegList& L, const ByteSource& B, const GelfKey& k, const GelfVal& v) {
+    L.text(k.name.p, k.name.len, k.esc);
+    if (v.tag == 0u) {
+        L.lit(L_MID, 3);  // ":"
+        L.text(B.at((int)(uint32_t)v.v), (int)(v.v >> 32), v.esc);
+        L.lit(L_QUOTE, 1);
+        return;
+    }
+    L.lit(L_MID, 2);  // ":
+    L.num(P.wentry_val + v.e, v.tag);
+}
+
+// serde_json 0.8 for the typed values of an LTSV or GELF record: Bool as true / false, F64 through dtoa (non-finite ->
+// null), I64 / U64 in decimal; kNull (GELF): FG_TAG_NULL as null
+template <bool kNull = false>
 __device__ __forceinline__ int json_number(unsigned long long v, uint32_t tag, uint8_t* out) {
+    if (kNull && tag == 5u) {
+        const uint32_t w = 0x6C6C756Eu;  // "null", low byte first
+        for (int k = 0; k < 4; ++k) out[k] = (uint8_t)(w >> (8 * k));
+        return 4;
+    }
     if (tag == 1u) {
         const uint32_t w = v ? 0x65757274u : 0x736C6166u;  // "true" / "fals", low byte first
         for (int k = 0; k < 4; ++k) out[k] = (uint8_t)(w >> (8 * k));
@@ -556,6 +717,8 @@ __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const 
                 first = false;
                 if constexpr (Src::kLtsv) {
                     ltsv_pair(P, L, B, bn, bv);
+                } else if constexpr (Src::kGelf) {
+                    gelf_pair(P, L, B, bn, bv);
                 } else {
                     L.push(bn.p, bn.len, true);
                     L.lit(L_MID, 3);  // ":"
@@ -567,7 +730,7 @@ __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const 
             }
         }
         if (tail) break;
-        const int kind = P.static_kind[si];
+        int kind = P.static_kind[si];
         if (live) {
             bool take = true;
             if (c == 0) {
@@ -580,12 +743,27 @@ __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const 
             }
             if (kind == GF_SDID && !r.has_sd) take = false;
             if (Src::kOptional && (kind == GF_APP || kind == GF_PROC || (kind == GF_LEVEL && r.severity == kNoSeverity))) take = false;
+            if constexpr (Src::kGelf) {
+                if (kind == GF_FULL && r.full.p == nullptr) take = false;
+            }
             if (take) {
                 // the literal is `,"key":` (for an extra `,"key":"value"`): the comma is skipped for the first item
                 const uint8_t* lit = P.static_blob + P.static_lit_off[si];
                 const int lit_len = P.static_lit_off[si + 1] - P.static_lit_off[si];
                 L.push(lit + (first ? 1 : 0), lit_len - (first ? 1 : 0), false);
                 first = false;
+                if constexpr (Src::kGelf) {  // the fixed string fields may hold JSON escapes
+                    switch (kind) {
+                        case GF_FULL: L.str_json(r.full, r.flags & kFullEsc); kind = -1; break;
+                        case GF_HOST:
+                            if (r.host.len) { L.str_json(r.host, r.flags & kHostEsc); kind = -1; }
+                            break;
+                        case GF_SHORT:
+                            if (r.msg.p) { L.str_json(r.msg, r.flags & kMsgEsc); kind = -1; }
+                            break;
+                        default: break;
+                    }
+                }
                 switch (kind) {  // warp-uniform
                     case GF_APP: L.str(r.app); break;
                     case GF_FULL: L.str(r.full); break;
@@ -610,12 +788,7 @@ __device__ __forceinline__ void build_segments(const GelfEncodeParams& P, const 
     if (live) L.lit(L_CLOSE, 1);
 }
 
-// serde_json 0.8 ser.rs escape_bytes: `"` `\` \b \f \n \r \t get a backslash form (returns the second byte), else 0
-__device__ __forceinline__ uint32_t json_escape_of(uint32_t c) {
-    if (c == '"' || c == '\\') return c;
-    if (c >= 0x20u) return 0u;
-    return c == 8u ? 'b' : c == 9u ? 't' : c == 10u ? 'n' : c == 12u ? 'f' : c == 13u ? 'r' : 0u;
-}
+// (json_escape_of, serde_json 0.8 ser.rs escape_bytes, lives in fg_gelf.cuh next to the decoder's unescape)
 
 // 0x80 in every byte of w that serde_json escapes: '"', '\\', or a byte below 0x20 (a superset of \b \f \n \r \t: the
 // other control bytes take the one-byte path and are copied there)
@@ -692,6 +865,67 @@ __device__ __forceinline__ void run_segments(const SegList& L, bool live, Sink& 
     }
 }
 
+// The same loop for a GELF record, whose list may also hold JSON string bodies (kJsonBit; `mode2` = the line went
+// through the newline retry): four source bytes per iteration while they hold no backslash and no byte to escape, else
+// one source escape (or byte) re-encoded by json_transcode_step, 1..4 output bytes.  Numbers as in run_segments<kNum>,
+// plus FG_TAG_NULL.  (A separate routine: any change to run_segments' template moves the register allocation of the
+// other three sources' kernels.)
+template <class Sink>
+__device__ __forceinline__ void run_json_segments(const SegList& L, bool live, Sink& s, bool mode2) {
+    int si = 0, k = 0, len = 0;
+    bool esc = false, json = false;
+    const uint8_t* p = nullptr;
+    uint32_t pending = 0;
+    bool more = live && L.n > 0;
+    uint8_t text[32];
+    auto enter = [&](const Seg& g) {
+        p = g.p;
+        len = g.len & ~(kEscBit | kJsonBit);
+        esc = g.len < 0;
+        json = (g.len & kJsonBit) != 0;
+        k = 0;
+        const unsigned long long* v = reinterpret_cast<const unsigned long long*>(p);
+        if (v >= s.vals && v < s.vals + s.cap) {  // no byte segment points into the value column
+            len = json_number<true>(*v, (uint32_t)len, text);
+            p = text;
+        }
+    };
+    if (more) enter(L.s[0]);
+    while (__any_sync(0xFFFFFFFFu, more)) {
+        if (more) {
+            uint32_t w;
+            int n = 1;
+            if (pending) {
+                w = pending;
+                pending = 0;
+            } else {
+                w = p[k];
+                if (k + 4 <= len) {
+                    const uint32_t w4 = w | ((uint32_t)p[k + 1] << 8) | ((uint32_t)p[k + 2] << 16) | ((uint32_t)p[k + 3] << 24);
+                    if (!esc || json_escape_flags4(w4) == 0u) {
+                        w = w4;
+                        n = 4;
+                    }
+                }
+                if (json && n == 1) {
+                    n = json_transcode_step(p, k, len, mode2, w);
+                } else {
+                    k += n;
+                    if (esc && n == 1) {
+                        const uint32_t e = json_escape_of(w);
+                        if (e) { pending = e; w = '\\'; }
+                    }
+                }
+            }
+            s.push(w, n);
+            if (k >= len && !pending) {  // next segment (none is empty)
+                if (++si < L.n) enter(L.s[si]);
+                else more = false;
+            }
+        }
+    }
+}
+
 // a record of any size: windows of kMaxSegs segments, every window through the warp-uniform loop
 template <class Src, class Sink>
 __device__ __forceinline__ void emit_record(const GelfEncodeParams& P, const ByteSource& B, const RecView& r, bool live, Sink& s) {
@@ -704,6 +938,9 @@ __device__ __forceinline__ void emit_record(const GelfEncodeParams& P, const Byt
         if constexpr (Src::kLtsv) {
             NumSink<Sink> ns{s, P.wentry_val, P.wentry_cap};
             run_segments<NumSink<Sink>, true>(L, live, ns);
+        } else if constexpr (Src::kGelf) {
+            NumSink<Sink> ns{s, P.wentry_val, P.wentry_cap};
+            run_json_segments(L, live, ns, (r.flags & kNlRetry) != 0u);
         } else {
             run_segments(L, live, s);
         }
@@ -850,7 +1087,9 @@ cudaError_t configure_gelf_encode(int max_tile_bytes) {
     if (e != cudaSuccess) return e;
     e = configure_src<From3164>(max_tile_bytes);
     if (e != cudaSuccess) return e;
-    return configure_src<FromLtsv>(max_tile_bytes);
+    e = configure_src<FromLtsv>(max_tile_bytes);
+    if (e != cudaSuccess) return e;
+    return configure_src<FromGelf>(max_tile_bytes);
 }
 
 size_t gelf_scan_temp_bytes(int n) {
@@ -864,6 +1103,7 @@ cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_
     switch (fmt) {
         case 0: return launch_src<From5424>(p, d_scan_temp, scan_temp_bytes, stream);
         case 1: return launch_src<FromLtsv>(p, d_scan_temp, scan_temp_bytes, stream);
+        case 2: return launch_src<FromGelf>(p, d_scan_temp, scan_temp_bytes, stream);
         case 3: return launch_src<From3164>(p, d_scan_temp, scan_temp_bytes, stream);
         default: return cudaErrorInvalidValue;
     }

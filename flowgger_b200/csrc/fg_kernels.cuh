@@ -138,7 +138,7 @@ cudaError_t launch_parse5424(const Parse5424Params& p, cudaStream_t stream, cuda
 cudaError_t configure_parse5424(int max_tile_bytes);
 int parse5424_smem_bytes(int tile_bytes);
 
-// ---- fused GELF encoder over the RFC5424, RFC3164 or LTSV results (fg_gelf_encode.cu) ---------------------------------
+// ---- fused GELF encoder over the RFC5424, RFC3164, LTSV or GELF results (fg_gelf_encode.cu) ---------------------------
 struct GelfEncodeParams {
     const uint8_t* bytes;
     const int32_t* offsets;  // [n+1], element 0 = first line of this launch
@@ -181,9 +181,15 @@ struct GelfEncodeParams {
     const uint8_t* ltsv_suffix;
     int32_t ltsv_suffix_off[6];
     int32_t* ltsv_stop;
+    // GELF source (col_sd as for LTSV): Record.ts of a row without "timestamp" (FG_FLAG_TS_MISSING), the wall clock read
+    // once per call (fg_encoded_gelf_now)
+    double gelf_now;
+    // rows the GELF parse kernels placed in the side table so far: past wentry_cap, a row's {first, count} may name
+    // rows of other lines (the batch is redone after the regrow), so no row is read
+    const uint32_t* gelf_entries;
 };
 cudaError_t configure_gelf_encode(int max_tile_bytes);
-// fmt: the decoder whose results the encoder reads (0 = RFC5424, 1 = LTSV, 3 = RFC3164)
+// fmt: the decoder whose results the encoder reads (0 = RFC5424, 1 = LTSV, 2 = GELF, 3 = RFC3164)
 cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
 size_t gelf_scan_temp_bytes(int n);
 

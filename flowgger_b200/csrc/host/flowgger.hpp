@@ -184,12 +184,15 @@ class Encoder {
 // encoder/gelf_encoder.rs:10-48: output.format = "gelf".  The encoder runs FUSED with the decoder on the GPU
 // (fg_decode_encode_gelf) for the input formats fuses_with() accepts: the batching splitters and RecordBatcher recognise
 // this type and never materialise Records for them (for LTSV they print the decoder's "Missing value" lines from
-// fg_encoded_ltsv_stops).
+// fg_encoded_ltsv_stops; GELF prints nothing, and its records without "timestamp" carry the wall clock of the call,
+// fg_encoded_gelf_now).
 class CudaGelfEncoder : public Encoder {
    public:
     explicit CudaGelfEncoder(std::vector<std::pair<std::string, std::string>> extra = {}) : extra_(std::move(extra)) {}
     // the decoders whose device-resident results the fused encoder reads (fg_decode_encode_gelf)
-    static bool fuses_with(fg_format fmt) { return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || fmt == FG_FMT_LTSV; }
+    static bool fuses_with(fg_format fmt) {
+        return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF;
+    }
     // a lone host-side Record cannot be encoded: there is no CPU encoder behind this interface
     bool encode(Record&&, std::vector<uint8_t>&, const char** err) const override {
         if (err) *err = "GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)";

@@ -106,6 +106,7 @@ def load_cuda() -> C.CDLL:
         L.fg_split_decode_encode_gelf.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.POINTER(FgEncodedOut),
                                                   C.POINTER(C.POINTER(C.c_int32))]
         L.fg_encoded_ltsv_stops.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
+        L.fg_encoded_gelf_now.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         _cuda = L
     return _cuda
 
@@ -356,12 +357,15 @@ class BatchDecoder:
         self._check(self.L.fg_set_gelf_extra(self.ctx, len(ex), keys, vals), "fg_set_gelf_extra")
 
     def decode_encode_gelf(self, data: np.ndarray, offsets: np.ndarray, copy: bool = True):
-        """decode + GelfEncoder::encode fused on the device, for a decoder of FMT_RFC5424, FMT_RFC3164 or FMT_LTSV (GELF
-        raises): (JSON bytes, int64 offsets[n+1], status uint8[n], kernel ms).  An RFC3164 record has no application_name,
+        """decode + GelfEncoder::encode fused on the device, for a decoder of FMT_RFC5424, FMT_RFC3164, FMT_LTSV or
+        FMT_GELF: (JSON bytes, int64 offsets[n+1], status uint8[n], kernel ms).  An RFC3164 record has no application_name,
         process_id or sd_id, "level" only when the line has a <PRI>, and always a "short_message" (possibly "").  An LTSV
         record has no application_name, process_id or sd_id, one "_" + name (+ type suffix) key per pair with typed
         values as JSON bools / numbers, and "-" as short_message without a `message` part; ltsv_stops() gives its
-        "Missing value" lines.  With copy=False the arrays are views of the context's pinned buffers (valid until the
+        "Missing value" lines.  A GELF record has no application_name, process_id or sd_id, "level" and
+        "full_message" only when the object has them, one "_" + name key per other member (the name alone when it starts
+        with "_"), strings re-escaped from their unescaped text, and gelf_now() as "timestamp" when the object has none.
+        With copy=False the arrays are views of the context's pinned buffers (valid until the
         next call)."""
         assert data.dtype == np.uint8 and offsets.dtype == np.int32
         out = FgEncodedOut()
@@ -378,7 +382,7 @@ class BatchDecoder:
         return buf, offs, status, out.kernel_ms
 
     def split_decode_encode_gelf(self, stream: np.ndarray, framing: int = 0, copy: bool = True):
-        """Framing (0 = "line", 1 = "nul") + UTF-8 validation + decode (FMT_RFC5424, FMT_RFC3164 or FMT_LTSV) + GelfEncoder::encode
+        """Framing (0 = "line", 1 = "nul") + UTF-8 validation + decode (FMT_RFC5424, FMT_RFC3164, FMT_LTSV or FMT_GELF) + GelfEncoder::encode
         of a raw byte stream, all on the device: (JSON bytes, int64 offsets[n+1], status uint8[n], record starts
         int32[n+1] in `stream` with their terminators, kernel ms).  A record that is not UTF-8 has status 76
         ("Invalid UTF-8 input") and an empty JSON record.
@@ -408,6 +412,13 @@ class BatchDecoder:
         self._check(self.L.fg_encoded_ltsv_stops(self.ctx, C.byref(p)), "fg_encoded_ltsv_stops")
         n = self._last_encoded_n
         return np.ctypeslib.as_array(p, shape=(n,)).copy() if n else np.zeros(0, np.int32)
+
+    def gelf_now(self) -> float:
+        """After decode_encode_gelf / split_decode_encode_gelf on a GELF decoder: the "timestamp" its records without one
+        were given, the wall clock read once at the start of that call (fg_encoded_gelf_now)."""
+        v = C.c_double()
+        self._check(self.L.fg_encoded_gelf_now(self.ctx, C.byref(v)), "fg_encoded_gelf_now")
+        return v.value
 
     def split_decode(self, stream: np.ndarray) -> BatchResult:
         """Framing + UTF-8 validation + decode of a raw newline-terminated byte stream, all on the device."""
@@ -572,7 +583,7 @@ def clone_decode_threads(fmt: int, lines: list[bytes], nthreads: int = 2, device
 def splitter_run_gelf(dec: "BatchDecoder", text: bytes, extra: dict[str, str] | None = None, max_lines: int = 1 << 16,
                       max_bytes: int = 16 << 20, framing: int = 0, stdout: bool = False) -> tuple[bytes, ...]:
     """BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or BatchingSyslenSplitter (framing 2: records
-    framed on the host and batched by RecordBatcher) with input.format = rfc5424, rfc3164 or ltsv (the decoder's format)
+    framed on the host and batched by RecordBatcher) with input.format = rfc5424, rfc3164, ltsv or gelf (the decoder's format)
     and output.format = gelf (decode and encode fused on the GPU, framing too for 0 and 1): returns (JSON records
     separated by newlines, stderr text), and with stdout=True also the stdout text (LTSV's "Missing value" lines)."""
     H = load_host()

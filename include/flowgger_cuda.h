@@ -254,8 +254,8 @@ int fg_flush_l2(fg_ctx* ctx); /* writes a >L2-sized scratch buffer */
 
 /* ---- decode + encode fused on the device (SURVEY.md 8(f) N2) ------------------------------------------------------
  * The reference calls Encoder::encode right after Decoder::decode for every record (splitter/line_splitter.rs:50-52).
- * For output.format = "gelf" with input.format = "rfc5424" (the default pair), "rfc3164" or "ltsv" both stages run on
- * the GPU and only the encoded records come back:
+ * For output.format = "gelf" with input.format = "rfc5424" (the default pair), "rfc3164", "ltsv" or "gelf" (a GELF
+ * relay) both stages run on the GPU and only the encoded records come back:
  *     GelfEncoder::new(&Config)   encoder/gelf_encoder.rs:29-48   -> fg_set_gelf_extra (output.gelf_extra)
  *     Encoder::encode(Record)     encoder/gelf_encoder.rs:59-115, encoder/mod.rs:54-56 -> fg_decode_encode_gelf
  * Record i is bytes[offsets[i], offsets[i+1]) — exactly the Vec<u8> the reference's encode returns (serde_json 0.8
@@ -267,8 +267,15 @@ int fg_flush_l2(fg_ctx* ctx); /* writes a >L2-sized scratch buffer */
  * application_name, process_id or sd_id, "level" only when the line has a `level` part, "short_message" "-" without a
  * `message` part and "" for `message:`, and one "_" + name (+ the type's suffix, input.ltsv_suffixes) key per pair: a
  * later pair of the same key replaces an earlier one, and a schema-typed value is written as a JSON bool or number
- * (non-finite f64 -> null).  GELF input, and LTSV input on a context not created for LTSV
- * (fg_config.input_format), -> FG_E_ARG. */
+ * (non-finite f64 -> null).  A GELF record (gelf_decoder.rs:34-125) has no application_name, process_id or sd_id,
+ * "version":"1.1" whatever version the input named, "level" and "full_message" only when the object has them,
+ * "short_message" "-" without one, "host" "unknown" for "", and one key per other member: "_" + its name, or the name
+ * alone when it starts with '_' (a later member of the same key, in the order of the input's sorted keys, replaces an
+ * earlier one); strings are written as serde_json escapes their unescaped text (`\/` -> `/`, `\u00e9` -> its UTF-8,
+ * control bytes other than \b \f \n \r \t raw), numbers, booleans and null as JSON.  A record without "timestamp"
+ * gets the wall clock read ONCE at the start of the call (fg_encoded_gelf_now), where the reference reads it per record
+ * as it decodes: the two differ by at most the duration of the call.  LTSV or GELF input on a context not created for
+ * that format (fg_config.input_format) -> FG_E_ARG. */
 typedef struct fg_encoded_out {
     int32_t n;
     const uint8_t* bytes;     /* concatenated records */
@@ -278,16 +285,16 @@ typedef struct fg_encoded_out {
     float total_ms;
 } fg_encoded_out;
 int fg_set_gelf_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
-int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV */, const uint8_t* bytes,
-                          const int32_t* offsets, int32_t n, fg_encoded_out* out);
-/* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424, RFC3164 or
- * LTSV decode -> GelfEncoder::encode, all on the device; only the encoded records and the record extents come back.
+int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */,
+                          const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
+/* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424, RFC3164,
+ * LTSV or GELF decode -> GelfEncoder::encode, all on the device; only the encoded records and the record extents come back.
  * Record i is out->bytes[out->offsets[i], out->offsets[i+1]); out->status[i] is 0, a decoder status, or the framing status
  * whose fg_error_string is "Invalid UTF-8 input" (empty record).  *line_offsets ([n+1], starts in `stream`, each record
  * still carrying its terminator, like fg_batch_out.line_offsets) stays valid until the next call on the context.
- * Errors: GELF input, LTSV input on a context not created for LTSV, or an unknown framing -> FG_E_ARG; nbytes > max_batch_bytes or more records than
- * max_batch_lines -> FG_E_CAPACITY (the context stays usable). */
-int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV */, fg_framing framing,
+ * Errors: LTSV or GELF input on a context not created for that format, or an unknown framing -> FG_E_ARG;
+ * nbytes > max_batch_bytes or more records than max_batch_lines -> FG_E_CAPACITY (the context stays usable). */
+int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */, fg_framing framing,
                                 const uint8_t* stream, int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
 /* The one side effect of LTSVDecoder::decode, println!("Missing value for name '{}'") for every tab-separated part
  * without ':' that the decode loop reached (ltsv_decoder.rs:99), for the records of the last fused call on an LTSV
@@ -297,6 +304,10 @@ int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | F
  * record that starts before that offset and holds no ':' prints one line, in order.  A record that is not UTF-8 has -1.
  * Returns FG_E_ARG when the last fused call was not on LTSV input or failed. */
 int fg_encoded_ltsv_stops(const fg_ctx* ctx, const int32_t** stop);
+/* Record.ts of every record without "timestamp" in the last fused call on GELF input: CLOCK_REALTIME at the start of
+ * that call, as secs + nanos / 1e9 (utils/mod.rs:16-21).  Returns FG_E_ARG when the last fused call was not on GELF
+ * input or failed. */
+int fg_encoded_gelf_now(const fg_ctx* ctx, double* now);
 
 /* the reference's Err(&'static str) for a row status (0 -> NULL) */
 const char* fg_error_string(fg_format fmt, uint32_t status);

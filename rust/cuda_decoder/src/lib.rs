@@ -217,7 +217,7 @@ impl CudaDecoder {
     }
 
     /// Framing + UTF-8 validation + decode + `GelfEncoder::encode` of a raw stream on the device
-    /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424", "rfc3164" or "ltsv", see `fuses_with_gelf`):
+    /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424", "rfc3164", "ltsv" or "gelf", see `fuses_with_gelf`):
     /// `f(line, Ok(json) | Err(error), side)` in stream order, `line` without its terminator, `side` the decoder's
     /// println! lines for it (LTSV's "Missing value" lines, from `fg_encoded_ltsv_stops`).  false (nothing decoded) when
     /// the stream does not fit the context.
@@ -583,14 +583,16 @@ impl<T: Read> Splitter<T> for BatchingLineSplitter {
 /// The `input.format` values whose decoder runs fused with the GELF encoder on the device (`fg_decode_encode_gelf`,
 /// `fg_split_decode_encode_gelf`); `FusedGelfLineSplitter` takes a `CudaDecoder` of one of them.
 pub fn fuses_with_gelf(input_format: &str) -> bool {
-    matches!(input_format, "rfc5424" | "rfc3164" | "ltsv")
+    matches!(input_format, "rfc5424" | "rfc3164" | "ltsv" | "gelf")
 }
 
-/// `output.format = "gelf"` with `input.format = "rfc5424"`, `"rfc3164"` or `"ltsv"` (`fuses_with_gelf`): framing, the
+/// `output.format = "gelf"` with `input.format = "rfc5424"`, `"rfc3164"`, `"ltsv"` or `"gelf"` (`fuses_with_gelf`): framing, the
 /// UTF-8 check, decode AND encode run on the device (`fg_split_decode_encode_gelf`, replaces BufRead::lines +
 /// Decoder::decode + GelfEncoder::encode of line_splitter.rs:17-52); it reads raw blocks like `BatchingLineSplitter` and
 /// only the encoded records come back.  An RFC3164 context fixes the year of year-less timestamps at the start of each
-/// call; an LTSV context's "Missing value" lines are printed to stdout before their record is sent or reported.
+/// call; an LTSV context's "Missing value" lines are printed to stdout before their record is sent or reported.  A GELF
+/// context (a GELF relay) stamps every record without "timestamp" with the wall clock read once at the start of each call
+/// (`fg_encoded_gelf_now`) rather than per record, and re-escapes strings from their unescaped text.
 pub struct FusedGelfLineSplitter {
     pub gpu: CudaDecoder,
     pub extra: Vec<(String, String)>,   // output.gelf_extra (gelf_encoder.rs:29-48)

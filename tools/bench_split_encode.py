@@ -1,14 +1,15 @@
 """Framing on the device vs on the host for the fused GELF pipelines (output.format = "gelf", input.format = "rfc5424",
-the default pair, "rfc3164" or "ltsv").
+the default pair, "rfc3164", "ltsv" or "gelf").
 
-    python tools/bench_split_encode.py [--format rfc5424|rfc3164|ltsv] [--ltsv-typed] [--lines 10000000] [--steps 10]
+    python tools/bench_split_encode.py [--format rfc5424|rfc3164|ltsv|gelf] [--ltsv-typed] [--lines 10000000] [--steps 10]
                                        [--warmup 2] [--splitter-gb 1.0] [--splitter-only]
 
 On the workload of bench.py for the format (rfc5424: C2, seed 5424; rfc3164: seed 3164, year 2026; ltsv: seed 1757,
-with --ltsv-typed bench.py's schema and suffixes; the same mean line length), joined with '\\n' in pinned memory:
+with --ltsv-typed bench.py's schema and suffixes; gelf: bench.py's seed; the same mean line length), joined with '\\n' in pinned memory:
   1. fg_split_decode_encode_gelf on the raw stream and fg_decode_encode_gelf on the same lines framed beforehand (for
-     rfc3164 and ltsv also fg_split_decode on the raw stream: decode only, rows + side tables back), timed alternately
-     after warm-ups; the two encoding calls must return byte-identical records, statuses and (ltsv) "Missing value" stops;
+     rfc3164, ltsv and gelf also fg_split_decode on the raw stream: decode only, rows + side tables back), timed alternately
+     after warm-ups; the two encoding calls must return byte-identical records, statuses and (ltsv) "Missing value" stops
+     (gelf: a record without "timestamp" carries its call's wall clock, which is swapped for the other call's first);
   2. the C++ BatchingLineSplitter with the fused GELF encoder end to end over at least --splitter-gb of the same text
      (text in, every JSON record handed to the sender, stderr captured).
 Prints one JSON line per section, with the card's name and power limit.  --splitter-only runs section 2 alone."""
@@ -31,7 +32,8 @@ import flowgger_b200 as fb  # noqa: E402
 
 # bench.py: SEEDS, GEN_MEAN and RFC3164_YEAR (the year of a timestamp without one, fixed so that a run is reproducible)
 WORKLOADS = {"rfc5424": (fb.FMT_RFC5424, 5424, 169.2), "rfc3164": (fb.FMT_RFC3164, 3164, 140.0),
-             "ltsv": (fb.FMT_LTSV, bench.SEEDS["ltsv"], bench.GEN_MEAN["ltsv"])}
+             "ltsv": (fb.FMT_LTSV, bench.SEEDS["ltsv"], bench.GEN_MEAN["ltsv"]),
+             "gelf": (fb.FMT_GELF, bench.SEEDS["gelf"], bench.GEN_MEAN["gelf"])}
 RFC3164_YEAR = 2026
 
 
@@ -49,6 +51,28 @@ def workload(fmt_name: str, n: int) -> tuple[np.ndarray, np.ndarray]:
     """the raw stream (every line followed by '\\n') and its line offsets, terminators included"""
     fmt, seed, mean = WORKLOADS[fmt_name]
     return fb.generate(fmt, seed, n, mean_len=mean, bad_frac=0.005, nthreads=32, terminated=True)
+
+
+def same_clock(res, sb, so, pb, po):
+    """GELF: the records of lines without "timestamp" carry the wall clock of their call.  Returns both calls' records
+    with the split call's clock text replaced by the pre-framed call's (one record shows each), as bytes + offsets."""
+    missing = np.flatnonzero(((res.meta & 0xFF) == 0) & (((res.meta >> 24) & 0x01) != 0))
+    sb, pb = bytes(sb), bytes(pb)
+    if len(missing) == 0:
+        return sb, so, pb, po
+    i = int(missing[0])
+
+    def clock(buf, offs):
+        rec = buf[offs[i]:offs[i + 1]]
+        a = rec.index(b',"timestamp":') + len(b',"timestamp":')
+        return rec[a:rec.index(b",", a)]  # "version" always follows
+
+    ts, tp = clock(sb, so), clock(pb, po)
+    sb = sb.replace(b',"timestamp":' + ts + b",", b',"timestamp":' + tp + b",")
+    grow = np.zeros(len(so), np.int64)
+    grow[missing + 1] = len(tp) - len(ts)
+    so = so + np.cumsum(grow)
+    return np.frombuffer(sb, np.uint8), so, np.frombuffer(pb, np.uint8), po
 
 
 def decoder(fmt_name: str, typed: bool = False, **kw) -> fb.BatchDecoder:
@@ -105,6 +129,8 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
         sb, so, ss, sl, _ = split.split_decode_encode_gelf(hs, copy=False)
         pb, po, ps, _ = pre.decode_encode_gelf(hl, ho, copy=False)
         assert len(ss) == n and np.array_equal(sl, soffs), "the device framed other lines than the generator made"
+        if args.format == "gelf":
+            sb, so, pb, po = same_clock(decode.split_decode(hd), sb, so, pb, po)
         assert np.array_equal(so, po) and np.array_equal(ss, ps) and np.array_equal(sb, pb), \
             "fg_split_decode_encode_gelf and fg_decode_encode_gelf disagree"
         if args.format == "ltsv":
