@@ -10,6 +10,10 @@ from .native import (  # noqa: F401
     FMT_LTSV,
     FMT_RFC3164,
     FMT_RFC5424,
+    OUT_LINE,
+    OUT_NONE,
+    OUT_NUL,
+    OUT_SYSLEN,
     BatchDecoder,
     BatchResult,
     NativeLibraryMissing,
@@ -26,6 +30,7 @@ from .native import (  # noqa: F401
     shard_by_bytes,
     splitter_run,
     splitter_run_gelf,
+    splitter_run_gelf_framed,
     tz_count,
     tz_lookup,
 )

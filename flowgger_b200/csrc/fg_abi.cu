@@ -237,6 +237,7 @@ struct fg_ctx {
     const int32_t* d_static_lit_off = nullptr;
     const int32_t* d_static_kind = nullptr;
     std::vector<std::pair<std::string, std::string>> gelf_extra;
+    fg_out_framing out_framing = FG_OUT_NONE;  // output.framing of the fused encoder (fg_set_output_framing)
     // split mode (fg_split_decode)
     Buf<uint32_t> seg;
     Buf<int32_t> n_lines;
@@ -636,6 +637,7 @@ int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream
     E.wide_cap = cap32(c, T_WIDE);
     E.wentry_cap = cap32(c, T_ENTRIES);
     E.arena_cap = cap32(c, T_ARENA);
+    E.out_framing = (int32_t)c->out_framing;
     // the encoder's CTAs take 256 lines (4 x the parse kernel's 64); configure_gelf_encode allowed max_tile5
     E.tile_bytes = std::min(4 * tile, c->max_tile5);
     FG_CUDA(c, fg::launch_gelf_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
@@ -1206,6 +1208,14 @@ int fg_set_gelf_extra(fg_ctx* c, int32_t n, const char* const* keys, const char*
     }
     FG_CUDA(c, cudaDeviceSynchronize());
     return build_static_items(c);
+}
+
+int fg_set_output_framing(fg_ctx* c, fg_out_framing framing) {
+    if (!c) return FG_E_ARG;
+    if (framing != FG_OUT_NONE && framing != FG_OUT_LINE && framing != FG_OUT_NUL && framing != FG_OUT_SYSLEN)
+        return fail(c, FG_E_ARG, "unknown output framing");
+    c->out_framing = framing;
+    return FG_OK;
 }
 
 // decode (RFC5424, RFC3164, LTSV or GELF) + GelfEncoder::encode fused: H2D lines -> parse kernels -> size / scan / write

@@ -28,7 +28,9 @@
 //   gelf_write_kernel  one thread per line writes its record; output bytes are assembled four at a time and stored as
 //                      aligned 32-bit words, so a record costs a quarter of the store instructions / L2 requests of a
 //                      byte-wise copy
-// Both kernels run ONE emit routine over a counting or a writing sink, so the two passes cannot disagree.
+// Both kernels run ONE emit routine over a counting or a writing sink, so the two passes cannot disagree.  output.framing
+// (fg_out_frame.cuh) is one runtime value: the size pass counts the frame into a record's length, the write pass stores
+// the frame around the record's place before the record is emitted into it.
 // All SD names start with '_' (rfc5424_decoder.rs:221), i.e. they sort before every fixed GELF key; the general merge
 // with the pre-sorted static items (fixed keys + extras, prepared on the host once) still compares full keys.
 #include <cub/device/device_scan.cuh>
@@ -38,6 +40,7 @@
 #include "fg_common.cuh"
 #include "fg_dtoa.cuh"
 #include "fg_gelf.cuh"
+#include "fg_out_frame.cuh"
 #include "fg_r5fast.cuh"
 #include "fg_status.h"
 #include "fg_tma.cuh"
@@ -433,9 +436,13 @@ __device__ __forceinline__ int cmp_sd_key(const GelfKey& a, Span b) {
 // The record sources the kernels are instantiated for.  kSd: the record may carry structured data.  kOptional:
 // application_name and process_id are None, and level is None without a severity.  kLtsv: pairs are LtsvKey / LtsvVal
 // (composed keys, typed values), and the size pass writes the "Missing value" stop of every line.  kGelf: pairs are
-// GelfKey / GelfVal, full_message may be None, and spans may hold JSON escapes.
+// GelfKey / GelfVal, full_message may be None, and spans may hold JSON escapes.  kWriteCtas: the CTAs per SM
+// gelf_write_kernel is allocated for (launch bounds; 0: ptxas's choice).  It holds each write kernel at the registers it
+// had before the output.framing code was added to it (From3164 48, FromGelf 64): without the bound, ptxas cut FromGelf to
+// 48 registers with 214 B of spill stores, 3-4 % slower on the GELF workload.
 struct From5424 {
     static constexpr bool kSd = true, kOptional = false, kLtsv = false, kGelf = false;
+    static constexpr int kWriteCtas = 0;
     using Key = Span;
     using Val = Span;
     static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view(P, B, i, r); }
@@ -446,6 +453,7 @@ struct From5424 {
 };
 struct From3164 {
     static constexpr bool kSd = false, kOptional = true, kLtsv = false, kGelf = false;
+    static constexpr int kWriteCtas = 5;
     using Key = Span;
     using Val = Span;
     static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_3164(P, B, i, r); }
@@ -456,6 +464,7 @@ struct From3164 {
 };
 struct FromLtsv {
     static constexpr bool kSd = true, kOptional = true, kLtsv = true, kGelf = false;
+    static constexpr int kWriteCtas = 0;
     using Key = LtsvKey;
     using Val = LtsvVal;
     static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_ltsv(P, B, i, r); }
@@ -466,6 +475,7 @@ struct FromLtsv {
 };
 struct FromGelf {
     static constexpr bool kSd = true, kOptional = true, kLtsv = false, kGelf = true;
+    static constexpr int kWriteCtas = 4;
     using Key = GelfKey;
     using Val = GelfVal;
     static __device__ __forceinline__ void load(const GelfEncodeParams& P, const ByteSource& B, int i, RecView& r) { load_view_gelf(P, B, i, r); }
@@ -965,6 +975,7 @@ struct EncShared {
     uint64_t mbar;
     uint32_t hist[kLenClasses];
     uint16_t perm[kEncLines];
+    uint8_t pre[kEncLines];  // write kernel, syslen: prefix length of each line of the CTA
 };
 
 __device__ __forceinline__ ByteSource stage_lines(const GelfEncodeParams& P, uint8_t* tile, uint64_t* mbar, int first, int last) {
@@ -1024,7 +1035,7 @@ __global__ void __launch_bounds__(kEncLines) gelf_size_kernel(const __grid_const
     CountSink s;
     emit_record<Src>(P, B, r, r.ok, s);
     if (!valid) return;
-    P.lens[i] = r.ok ? s.n : 0ull;
+    P.lens[i] = r.ok ? framed_len(s.n, P.out_framing) : 0ull;
     P.status[i] = (uint8_t)Src::status(P, i);
     if constexpr (Src::kLtsv) P.ltsv_stop[i] = ltsv_stop(P, i);
 }
@@ -1037,13 +1048,22 @@ __global__ void gelf_base_kernel(const __grid_constant__ GelfEncodeParams P) {
 }
 
 template <class Src>
-__global__ void __launch_bounds__(kEncLines) gelf_write_kernel(const __grid_constant__ GelfEncodeParams P) {
+__global__ void __launch_bounds__(kEncLines, Src::kWriteCtas) gelf_write_kernel(const __grid_constant__ GelfEncodeParams P) {
     extern __shared__ __align__(128) uint8_t tile[];
     __shared__ __align__(8) EncShared sh;
     if (*P.bad_offsets) return;
     const int first = blockIdx.x * kEncLines, last = min(P.n, first + kEncLines);
+    if (P.out_framing != kOutNone && first + (int)threadIdx.x < last) {
+        // output.framing of line first + tid, stored before any record of the CTA is emitted (a record's own bytes lie
+        // strictly between its prefix and its suffix) and before the lines are sorted: none of it is live in the byte loop
+        const int j = first + (int)threadIdx.x;
+        const unsigned long long fl = P.lens[j], a = P.base[0] + P.rel[j];
+        uint32_t pre = 0;
+        if (fl != 0ull && a + fl <= P.out_cap) pre = (uint32_t)(frame_record(P.out_framing, fl, P.out + a) - (P.out + a));
+        sh.pre[threadIdx.x] = (uint8_t)pre;
+    }
     const ByteSource B = stage_lines(P, tile, &sh.mbar, first, last);
-    const int i = sorted_line(P, sh, first, last);
+    const int i = sorted_line(P, sh, first, last);  // (its barriers publish sh.pre)
     const bool valid = i >= 0;
     unsigned long long at = 0, len = 0;
     if (valid) {
@@ -1057,7 +1077,7 @@ __global__ void __launch_bounds__(kEncLines) gelf_write_kernel(const __grid_cons
     RecView r;
     r.ok = false;
     if (live) Src::load(P, B, i, r);
-    WordSink s(P.out + at);
+    WordSink s(P.out + at + (live && P.out_framing == kOutSyslen ? sh.pre[i - first] : 0));
     emit_record<Src>(P, B, r, live && r.ok, s);
 }
 

@@ -156,7 +156,7 @@ struct GelfEncodeParams {
     const int32_t* static_key_off;  // [n_static+1] raw key bytes (for ordering against the SD names)
     const int32_t* static_lit_off;  // [n_static+1] text to emit: `"key":`, for an extra `"key":"value"`
     const int32_t* static_kind;     // [n_static] GF_*
-    unsigned long long* lens;       // [n] record lengths (size pass)
+    unsigned long long* lens;       // [n] record lengths with their output.framing bytes (size pass)
     unsigned long long* rel;        // [n] exclusive sum of lens inside this launch
     unsigned long long* base;       // base[0] = output bytes before this launch, base[1] receives base[0] + this launch's bytes
     uint8_t* out;
@@ -187,6 +187,8 @@ struct GelfEncodeParams {
     // rows the GELF parse kernels placed in the side table so far: past wentry_cap, a row's {first, count} may name
     // rows of other lines (the batch is redone after the regrow), so no row is read
     const uint32_t* gelf_entries;
+    // output.framing (fg_out_frame.cuh: OutFraming) applied to every record written
+    int32_t out_framing;
 };
 cudaError_t configure_gelf_encode(int max_tile_bytes);
 // fmt: the decoder whose results the encoder reads (0 = RFC5424, 1 = LTSV, 2 = GELF, 3 = RFC3164)

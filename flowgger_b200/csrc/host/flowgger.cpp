@@ -225,7 +225,10 @@ void CudaBatchDecoder::decode_batch(const uint8_t* bytes, const int32_t* offsets
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_batch: ") + fg_last_error(ctx_));
 }
 
-void CudaBatchDecoder::set_gelf_extra(const std::vector<std::pair<std::string, std::string>>& extra) {
+void CudaBatchDecoder::set_encoder(const std::vector<std::pair<std::string, std::string>>& extra, fg_out_framing out_framing) {
+    // set on every call: a host-side setting, and other callers of the same context may have changed it
+    if (fg_set_output_framing(ctx_, out_framing) != FG_OK)
+        throw std::runtime_error(std::string("fg_set_output_framing: ") + fg_last_error(ctx_));
     if (extra_valid_ && extra == extra_set_) return;
     std::vector<const char*> k, v;
     for (const auto& kv : extra) {
@@ -239,8 +242,9 @@ void CudaBatchDecoder::set_gelf_extra(const std::vector<std::pair<std::string, s
 }
 
 void CudaBatchDecoder::decode_encode_gelf(const uint8_t* bytes, const int32_t* offsets, int32_t n,
-                                          const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out) {
-    set_gelf_extra(extra);
+                                          const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out,
+                                          fg_out_framing out_framing) {
+    set_encoder(extra, out_framing);
     const int rc = fg_decode_encode_gelf(ctx_, fmt_, bytes, offsets, n, out);
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_encode_gelf: ") + fg_last_error(ctx_));
 }
@@ -252,8 +256,8 @@ const int32_t* CudaBatchDecoder::encoded_ltsv_stops() const {
 
 bool CudaBatchDecoder::try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
                                                     const std::vector<std::pair<std::string, std::string>>& extra,
-                                                    fg_encoded_out* out, const int32_t** line_offsets) {
-    set_gelf_extra(extra);
+                                                    fg_encoded_out* out, const int32_t** line_offsets, fg_out_framing out_framing) {
+    set_encoder(extra, out_framing);
     const int rc = fg_split_decode_encode_gelf(ctx_, fmt_, framing, stream, nbytes, out, line_offsets);
     if (rc == FG_E_CAPACITY) return false;
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_split_decode_encode_gelf: ") + fg_last_error(ctx_));
@@ -534,7 +538,8 @@ void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
     if (fused_ != nullptr && CudaGelfEncoder::fuses_with(gpu->format())) {
         // decode + encode on the device (line_splitter.rs:50-52 fused): only the encoded records come back
         fg_encoded_out eo;
-        gpu->decode_encode_gelf(bytes, offsets_.data(), n, fused_->extra(), &eo);
+        const bool framed = fused_->out_framing() != FG_OUT_NONE;  // one buffer for the batch: the Output's bytes
+        gpu->decode_encode_gelf(bytes, offsets_.data(), n, fused_->extra(), &eo, fused_->out_framing());
         const int32_t* stops = gpu->encoded_ltsv_stops();
         std::vector<std::string> fx;
         for (int32_t i = 0; i < n; ++i) {
@@ -545,10 +550,14 @@ void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
                 ltsv_missing_values(bytes, lo, offsets_[(size_t)i + 1], lo + stops[i], fx);
                 for (const auto& s : fx) out_ << s << "\n";
             }
-            if (eo.status[i] == 0) tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
-            else report(fg_error_string(gpu->format(), eo.status[i]),
-                        std::string_view((const char*)bytes + offsets_[(size_t)i], (size_t)(offsets_[(size_t)i + 1] - offsets_[(size_t)i])));
+            if (eo.status[i] == 0) {
+                if (!framed) tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
+            } else {
+                report(fg_error_string(gpu->format(), eo.status[i]),
+                       std::string_view((const char*)bytes + offsets_[(size_t)i], (size_t)(offsets_[(size_t)i + 1] - offsets_[(size_t)i])));
+            }
         }
+        if (framed && eo.offsets[n] > 0) tx_(std::vector<uint8_t>(eo.bytes, eo.bytes + eo.offsets[n]));
     } else {
         fg_batch_out out;
         gpu->decode_batch(bytes, offsets_.data(), n, &out);
@@ -670,7 +679,8 @@ class BlockSplitter {
             // framing + decode + encode on the device (line_splitter.rs:17-52 fused): only the encoded records come back
             fg_encoded_out eo;
             const int32_t* lines;
-            if (!gpu->try_split_decode_encode_gelf(p, n, framing_, fused_->extra(), &eo, &lines)) return false;
+            const bool framed = fused_->out_framing() != FG_OUT_NONE;  // one buffer for the block: the Output's bytes
+            if (!gpu->try_split_decode_encode_gelf(p, n, framing_, fused_->extra(), &eo, &lines, fused_->out_framing())) return false;
             const int32_t* stops = gpu->encoded_ltsv_stops();
             std::vector<std::string> fx;
             for (int32_t i = 0; i < eo.n; ++i) {
@@ -682,11 +692,12 @@ class BlockSplitter {
                     for (const auto& s : fx) out_ << s << "\n";
                 }
                 if (eo.status[i] == 0) {
-                    tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
+                    if (!framed) tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
                     continue;
                 }
                 reject(fmt, eo.status[i], fg_error_string(fmt, eo.status[i]), p, lo, hi);
             }
+            if (framed && eo.offsets[eo.n] > 0) tx_(std::vector<uint8_t>(eo.bytes, eo.bytes + eo.offsets[eo.n]));
             return true;
         }
         fg_batch_out out;
@@ -1159,12 +1170,15 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
     }
 }
 
-// BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or BatchingSyslenSplitter (framing 2, through
-// RecordBatcher) with output.format = "gelf" (fused decode + encode): text in, one JSON record per line, stderr and
-// stdout text out
-int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
-                          const char* const* keys, const char* const* vals, uint8_t** out_records, int64_t* out_records_len,
-                          uint8_t** out_stderr, int64_t* out_stderr_len, int framing, uint8_t** out_stdout, int64_t* out_stdout_len) {
+}  // extern "C"
+
+namespace {
+
+// The harness of the two gelf splitter entries: BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or
+// BatchingSyslenSplitter (framing 2, through RecordBatcher) over `text` with `enc`; `tx` receives what the splitter sends
+int run_gelf_splitter(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int framing,
+                      const CudaGelfEncoder& enc, const std::function<void(std::vector<uint8_t>&&)>& tx, std::string& err,
+                      std::string& out) {
     struct Shared : Decoder {
         std::shared_ptr<CudaBatchDecoder> b;
         DecodeResult decode(std::string_view) const override { return {}; }
@@ -1172,32 +1186,69 @@ int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max
         std::shared_ptr<CudaBatchDecoder> batch() const override { return b; }
     } dec;
     dec.b = std::shared_ptr<CudaBatchDecoder>((CudaBatchDecoder*)d, [](CudaBatchDecoder*) {});
-    std::vector<std::pair<std::string, std::string>> extra;
-    for (int k = 0; k < n_extra; ++k) extra.emplace_back(keys[k], vals[k]);
-    CudaGelfEncoder enc(extra);
     BatchingLineSplitter::Limits lim;
     lim.max_lines = max_lines;
     lim.max_bytes = max_bytes;
     std::string in((const char*)text, (size_t)len);
     std::istringstream is(in);
     std::ostringstream es, os;
-    std::string records;
     try {
-        auto tx = [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); };
         if (framing == 1) BatchingNulSplitter(lim).run(is, tx, dec, enc, es, os);        // input.framing = "nul"
         else if (framing == 2) BatchingSyslenSplitter(lim).run(is, tx, dec, enc, es, os);  // input.framing = "syslen"
         else BatchingLineSplitter(lim).run(is, tx, dec, enc, es, os);
     } catch (const std::exception&) {
         return -1;
     }
-    auto give = [](const std::string& s, uint8_t** p, int64_t* n) {
-        *p = (uint8_t*)malloc(s.size() ? s.size() : 1);
-        memcpy(*p, s.data(), s.size());
-        *n = (int64_t)s.size();
-    };
+    err = es.str();
+    out = os.str();
+    return 0;
+}
+
+std::vector<std::pair<std::string, std::string>> extra_of(int n_extra, const char* const* keys, const char* const* vals) {
+    std::vector<std::pair<std::string, std::string>> extra;
+    for (int k = 0; k < n_extra; ++k) extra.emplace_back(keys[k], vals[k]);
+    return extra;
+}
+
+void give(const std::string& s, uint8_t** p, int64_t* n) {
+    *p = (uint8_t*)malloc(s.size() ? s.size() : 1);
+    memcpy(*p, s.data(), s.size());
+    *n = (int64_t)s.size();
+}
+
+}  // namespace
+
+extern "C" {
+
+// BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or BatchingSyslenSplitter (framing 2, through
+// RecordBatcher) with output.format = "gelf" (fused decode + encode): text in, one JSON record per line, stderr and
+// stdout text out
+int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
+                          const char* const* keys, const char* const* vals, uint8_t** out_records, int64_t* out_records_len,
+                          uint8_t** out_stderr, int64_t* out_stderr_len, int framing, uint8_t** out_stdout, int64_t* out_stdout_len) {
+    std::string records, err, out;
+    auto tx = [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); };
+    if (run_gelf_splitter(d, text, len, max_lines, max_bytes, framing, CudaGelfEncoder(extra_of(n_extra, keys, vals)), tx, err, out))
+        return -1;
     give(records, out_records, out_records_len);
-    give(es.str(), out_stderr, out_stderr_len);
-    give(os.str(), out_stdout, out_stdout_len);
+    give(err, out_stderr, out_stderr_len);
+    give(out, out_stdout, out_stdout_len);
+    return 0;
+}
+
+// fgh_splitter_run_gelf with output.framing (fg_out_framing) applied on the device: the output stream exactly as the
+// splitter sent it (no separator added), stderr and stdout text
+int fgh_splitter_run_gelf_framed(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
+                                 const char* const* keys, const char* const* vals, int framing, int out_framing, uint8_t** out_stream,
+                                 int64_t* out_stream_len, uint8_t** out_stderr, int64_t* out_stderr_len, uint8_t** out_stdout,
+                                 int64_t* out_stdout_len) {
+    std::string stream, err, out;
+    auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
+    const CudaGelfEncoder enc(extra_of(n_extra, keys, vals), (fg_out_framing)out_framing);
+    if (run_gelf_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
+    give(stream, out_stream, out_stream_len);
+    give(err, out_stderr, out_stderr_len);
+    give(out, out_stdout, out_stdout_len);
     return 0;
 }
 

@@ -115,19 +115,21 @@ class CudaBatchDecoder {
     void split_decode(const uint8_t* stream, int64_t nbytes, fg_batch_out* out, fg_framing framing = FG_FRAME_LINE);
     // the same, but false (nothing decoded) when the stream does not fit the context: more bytes or more records
     bool try_split_decode(const uint8_t* stream, int64_t nbytes, fg_batch_out* out, fg_framing framing);
-    // decode + GelfEncoder::encode fused on the device (fg_decode_encode_gelf); `extra` = output.gelf_extra
+    // decode + GelfEncoder::encode fused on the device (fg_decode_encode_gelf); `extra` = output.gelf_extra, `out_framing`
+    // = output.framing (fg_set_output_framing)
     void decode_encode_gelf(const uint8_t* bytes, const int32_t* offsets, int32_t n,
-                            const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out);
+                            const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out,
+                            fg_out_framing out_framing = FG_OUT_NONE);
     // framing + decode + GelfEncoder::encode fused on the device (fg_split_decode_encode_gelf); false as try_split_decode
     bool try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
                                       const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out,
-                                      const int32_t** line_offsets);
+                                      const int32_t** line_offsets, fg_out_framing out_framing = FG_OUT_NONE);
     // after one of the two fused calls on an LTSV context: where each record's "Missing value" lines stop
     // (fg_encoded_ltsv_stops, for ltsv_missing_values); nullptr for other formats
     const int32_t* encoded_ltsv_stops() const;
 
    private:
-    void set_gelf_extra(const std::vector<std::pair<std::string, std::string>>& extra);
+    void set_encoder(const std::vector<std::pair<std::string, std::string>>& extra, fg_out_framing out_framing);
     fg_format fmt_;
     fg_ctx* ctx_ = nullptr;
     std::mutex mu_;
@@ -185,10 +187,13 @@ class Encoder {
 // (fg_decode_encode_gelf) for the input formats fuses_with() accepts: the batching splitters and RecordBatcher recognise
 // this type and never materialise Records for them (for LTSV they print the decoder's "Missing value" lines from
 // fg_encoded_ltsv_stops; GELF prints nothing, and its records without "timestamp" carry the wall clock of the call,
-// fg_encoded_gelf_now).
+// fg_encoded_gelf_now).  `out_framing` = output.framing, applied on the device as well (fg_set_output_framing): with a
+// framing other than FG_OUT_NONE the fused paths send ONE buffer per device call, the framed records of the whole
+// batch, exactly what the Output writes, and the Output gets no merger.
 class CudaGelfEncoder : public Encoder {
    public:
-    explicit CudaGelfEncoder(std::vector<std::pair<std::string, std::string>> extra = {}) : extra_(std::move(extra)) {}
+    explicit CudaGelfEncoder(std::vector<std::pair<std::string, std::string>> extra = {}, fg_out_framing out_framing = FG_OUT_NONE)
+        : extra_(std::move(extra)), out_framing_(out_framing) {}
     // the decoders whose device-resident results the fused encoder reads (fg_decode_encode_gelf)
     static bool fuses_with(fg_format fmt) {
         return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF;
@@ -199,9 +204,11 @@ class CudaGelfEncoder : public Encoder {
         return false;
     }
     const std::vector<std::pair<std::string, std::string>>& extra() const { return extra_; }
+    fg_out_framing out_framing() const { return out_framing_; }
 
    private:
     std::vector<std::pair<std::string, std::string>> extra_;
+    fg_out_framing out_framing_;
 };
 
 // The batching twin of the reference's per-record call sites (`decode -> encode -> tx.send`, or print

@@ -11,6 +11,8 @@ LIB_DIR = Path(__file__).resolve().parent / "lib"
 
 FMT_RFC5424, FMT_LTSV, FMT_GELF, FMT_RFC3164 = 0, 1, 2, 3
 FMT_NAMES = {FMT_RFC5424: "rfc5424", FMT_LTSV: "ltsv", FMT_GELF: "gelf", FMT_RFC3164: "rfc3164"}
+# output.framing of the fused encoder (fg_out_framing)
+OUT_NONE, OUT_LINE, OUT_NUL, OUT_SYSLEN = 0, 1, 2, 3
 
 
 class NativeLibraryMissing(ImportError):
@@ -107,6 +109,7 @@ def load_cuda() -> C.CDLL:
                                                   C.POINTER(C.POINTER(C.c_int32))]
         L.fg_encoded_ltsv_stops.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
         L.fg_encoded_gelf_now.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        L.fg_set_output_framing.argtypes = [C.c_void_p, C.c_int]
         _cuda = L
     return _cuda
 
@@ -143,6 +146,8 @@ def load_host() -> C.CDLL:
         L.fgh_splitter_run_gelf.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int64, C.c_int, C.POINTER(C.c_char_p),
                                             C.POINTER(C.c_char_p)] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 2 + [C.c_int] + [
                                             C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
+        L.fgh_splitter_run_gelf_framed.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int64, C.c_int, C.POINTER(C.c_char_p),
+                                                   C.POINTER(C.c_char_p), C.c_int, C.c_int] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         L.fgh_splitter_run.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int64, C.c_int32, C.c_int64] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         _host = L
     return _host
@@ -355,6 +360,12 @@ class BatchDecoder:
         keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])
         vals = (C.c_char_p * max(len(ex), 1))(*[v.encode() for _, v in ex])
         self._check(self.L.fg_set_gelf_extra(self.ctx, len(ex), keys, vals), "fg_set_gelf_extra")
+
+    def set_output_framing(self, framing: int) -> None:
+        """output.framing of the fused calls (fg_set_output_framing): OUT_NONE, OUT_LINE ("\\n" after each record), OUT_NUL
+        ("\\0" after each record) or OUT_SYSLEN ("{len + 1} " before, "\\n" after).  A rejected record stays empty, so the
+        bytes of a fused call are the whole output stream of its batch."""
+        self._check(self.L.fg_set_output_framing(self.ctx, framing), "fg_set_output_framing")
 
     def decode_encode_gelf(self, data: np.ndarray, offsets: np.ndarray, copy: bool = True):
         """decode + GelfEncoder::encode fused on the device, for a decoder of FMT_RFC5424, FMT_RFC3164, FMT_LTSV or
@@ -601,6 +612,29 @@ def splitter_run_gelf(dec: "BatchDecoder", text: bytes, extra: dict[str, str] | 
         out.append(C.string_at(p, n.value))
         H.fgh_free(p)
     return tuple(out) if stdout else tuple(out[:2])
+
+
+def splitter_run_gelf_framed(dec: "BatchDecoder", text: bytes, out_framing: int, extra: dict[str, str] | None = None,
+                             max_lines: int = 1 << 16, max_bytes: int = 16 << 20, framing: int = 0) -> tuple[bytes, bytes, bytes]:
+    """splitter_run_gelf with output.framing applied on the device (OUT_NONE, OUT_LINE, OUT_NUL or OUT_SYSLEN): returns
+    (the output stream exactly as the splitter sent it, stderr text, stdout text)."""
+    H = load_host()
+    ex = list((extra or {}).items())
+    keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])
+    vals = (C.c_char_p * max(len(ex), 1))(*[v.encode() for _, v in ex])
+    ps = [C.c_void_p() for _ in range(3)]
+    ns = [C.c_int64() for _ in range(3)]
+    args = []
+    for p, n in zip(ps, ns):
+        args += [C.byref(p), C.byref(n)]
+    rc = H.fgh_splitter_run_gelf_framed(dec._h, text, len(text), max_lines, max_bytes, len(ex), keys, vals, framing, out_framing, *args)
+    if rc != 0:
+        raise RuntimeError("splitter failed")
+    out = []
+    for p, n in zip(ps, ns):
+        out.append(C.string_at(p, n.value))
+        H.fgh_free(p)
+    return tuple(out)
 
 
 def splitter_run(dec: "BatchDecoder", text: bytes, max_lines: int = 1 << 16, max_bytes: int = 16 << 20,

@@ -278,13 +278,25 @@ int fg_flush_l2(fg_ctx* ctx); /* writes a >L2-sized scratch buffer */
  * that format (fg_config.input_format) -> FG_E_ARG. */
 typedef struct fg_encoded_out {
     int32_t n;
-    const uint8_t* bytes;     /* concatenated records */
+    const uint8_t* bytes;     /* concatenated records, each framed by fg_set_output_framing */
     const int64_t* offsets;   /* [n+1] */
     const uint8_t* status;    /* [n] */
     float kernel_ms;          /* parse + encode kernels */
     float total_ms;
 } fg_encoded_out;
 int fg_set_gelf_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
+/* output.framing: the Merger the Output applies to every encoded record before it writes it (src/flowgger/merger; picked
+ * from output.framing in mod.rs:444-460; the caller resolves the reference's default and passes it here, as
+ * fg_set_gelf_extra stands for GelfEncoder::new).  From the next fused call on, record i of fg_encoded_out is the bytes
+ * the Output writes for it:
+ *     FG_OUT_NONE    the record (the default; "noop" / "nop" / "none" / "capnp")
+ *     FG_OUT_LINE    record "\n"                    (line_merger.rs:14)
+ *     FG_OUT_NUL     record "\0"                    (nul_merger.rs:14)
+ *     FG_OUT_SYSLEN  "{L + 1} " record "\n"          (syslen_merger.rs:15-28, L = the record's length in decimal)
+ * A rejected record stays empty (no frame), so bytes[0, offsets[n]) is the whole output stream of the call, in input
+ * order.  An unknown value -> FG_E_ARG, the context unchanged. */
+typedef enum fg_out_framing { FG_OUT_NONE = 0, FG_OUT_LINE = 1, FG_OUT_NUL = 2, FG_OUT_SYSLEN = 3 } fg_out_framing;
+int fg_set_output_framing(fg_ctx* ctx, fg_out_framing framing);
 int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */,
                           const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
 /* Raw stream -> framing (FG_FRAME_LINE | FG_FRAME_NUL, as fg_split_decode_framed) -> UTF-8 check -> RFC5424, RFC3164,

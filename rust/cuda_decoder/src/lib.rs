@@ -219,11 +219,13 @@ impl CudaDecoder {
     /// Framing + UTF-8 validation + decode + `GelfEncoder::encode` of a raw stream on the device
     /// (`fg_split_decode_encode_gelf`, input.format = "rfc5424", "rfc3164", "ltsv" or "gelf", see `fuses_with_gelf`):
     /// `f(line, Ok(json) | Err(error), side)` in stream order, `line` without its terminator, `side` the decoder's
-    /// println! lines for it (LTSV's "Missing value" lines, from `fg_encoded_ltsv_stops`).  false (nothing decoded) when
-    /// the stream does not fit the context.
-    pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String])>(&self, stream: &[u8],
-                                                                                             extra: &[(String, String)], mut f: F) -> bool {
+    /// println! lines for it (LTSV's "Missing value" lines, from `fg_encoded_ltsv_stops`); `json` carries the frame of
+    /// `out_framing` (output.framing, `fg_set_output_framing`).  Then `all(bytes)` with the framed records of the whole
+    /// call, the bytes one Output writes for them.  false (nothing decoded) when the stream does not fit the context.
+    pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String]), G: FnOnce(&[u8])>(
+        &self, stream: &[u8], extra: &[(String, String)], out_framing: fg_out_framing, mut f: F, all: G) -> bool {
         let mut ctx = self.ctx.lock().unwrap();
+        assert_eq!(unsafe { fg_set_output_framing(ctx.raw, out_framing) }, 0);
         if ctx.extra.as_deref() != Some(extra) {
             let keys: Vec<CString> = extra.iter().map(|(k, _)| CString::new(k.as_str()).unwrap()).collect();
             let vals: Vec<CString> = extra.iter().map(|(_, v)| CString::new(v.as_str()).unwrap()).collect();
@@ -267,6 +269,7 @@ impl CudaDecoder {
                 f(&stream[lo..hi], Err(error_str(ctx.fmt, st as u32)), &side);
             }
         }
+        all(unsafe { std::slice::from_raw_parts(out.bytes, *out.offsets.add(n) as usize) });
         true
     }
 }
@@ -586,6 +589,18 @@ pub fn fuses_with_gelf(input_format: &str) -> bool {
     matches!(input_format, "rfc5424" | "rfc3164" | "ltsv" | "gelf")
 }
 
+/// The device framing of an `output.framing` value, as `mod.rs:453-460` picks the merger (panics on an unknown one, as
+/// the reference does)
+pub fn out_framing_of(output_framing: &str) -> fg_out_framing {
+    match output_framing {
+        "noop" | "nop" | "none" | "capnp" => fg_out_framing_FG_OUT_NONE,
+        "line" => fg_out_framing_FG_OUT_LINE,
+        "nul" => fg_out_framing_FG_OUT_NUL,
+        "syslen" => fg_out_framing_FG_OUT_SYSLEN,
+        _ => panic!("Invalid framing type: {}", output_framing),
+    }
+}
+
 /// `output.format = "gelf"` with `input.format = "rfc5424"`, `"rfc3164"`, `"ltsv"` or `"gelf"` (`fuses_with_gelf`): framing, the
 /// UTF-8 check, decode AND encode run on the device (`fg_split_decode_encode_gelf`, replaces BufRead::lines +
 /// Decoder::decode + GelfEncoder::encode of line_splitter.rs:17-52); it reads raw blocks like `BatchingLineSplitter` and
@@ -593,25 +608,29 @@ pub fn fuses_with_gelf(input_format: &str) -> bool {
 /// call; an LTSV context's "Missing value" lines are printed to stdout before their record is sent or reported.  A GELF
 /// context (a GELF relay) stamps every record without "timestamp" with the wall clock read once at the start of each call
 /// (`fg_encoded_gelf_now`) rather than per record, and re-escapes strings from their unescaped text.
+/// With `out_framing` other than `FG_OUT_NONE` the device also applies output.framing (merger/*.rs) and the splitter
+/// sends ONE `Vec` per block, the framed records of the whole block: the Output must then be started without a merger.
 pub struct FusedGelfLineSplitter {
     pub gpu: CudaDecoder,
     pub extra: Vec<(String, String)>,   // output.gelf_extra (gelf_encoder.rs:29-48)
+    pub out_framing: fg_out_framing,    // output.framing (mod.rs:444-460), resolved by the caller
     pub max_bytes: usize,
 }
 
 impl<T: Read> Splitter<T> for FusedGelfLineSplitter {
     fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
         let max_bytes = self.max_bytes.min(self.gpu.capacity_bytes());
+        let framed = self.out_framing != fg_out_framing_FG_OUT_NONE;
         run_blocks(buf_reader, max_bytes, |block| {
             decode_fitting(&self.gpu, block, &mut |gpu: &CudaDecoder, part: &[u8]| {
-                gpu.split_decode_encode_gelf(part, &self.extra, |line, r, side| {
+                gpu.split_decode_encode_gelf(part, &self.extra, self.out_framing, |line, r, side| {
                     for s in side { println!("{}", s); }  // ltsv_decoder.rs:99
                     match r {
-                        Ok(json) => tx.send(json.to_vec()).unwrap(),
+                        Ok(json) => if !framed { tx.send(json.to_vec()).unwrap() },
                         Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
                         Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
                     }
-                })
+                }, |all| if framed && !all.is_empty() { tx.send(all.to_vec()).unwrap() })
             })
         });
     }

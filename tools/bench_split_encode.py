@@ -2,7 +2,7 @@
 the default pair, "rfc3164", "ltsv" or "gelf").
 
     python tools/bench_split_encode.py [--format rfc5424|rfc3164|ltsv|gelf] [--ltsv-typed] [--lines 10000000] [--steps 10]
-                                       [--warmup 2] [--splitter-gb 1.0] [--splitter-only]
+                                       [--warmup 2] [--splitter-gb 1.0] [--splitter-only] [--out-framing none|line|nul|syslen]
 
 On the workload of bench.py for the format (rfc5424: C2, seed 5424; rfc3164: seed 3164, year 2026; ltsv: seed 1757,
 with --ltsv-typed bench.py's schema and suffixes; gelf: bench.py's seed; the same mean line length), joined with '\\n' in pinned memory:
@@ -12,6 +12,8 @@ with --ltsv-typed bench.py's schema and suffixes; gelf: bench.py's seed; the sam
      (gelf: a record without "timestamp" carries its call's wall clock, which is swapped for the other call's first);
   2. the C++ BatchingLineSplitter with the fused GELF encoder end to end over at least --splitter-gb of the same text
      (text in, every JSON record handed to the sender, stderr captured).
+--out-framing applies output.framing on the device (fg_set_output_framing) in both sections: the encoding calls return the
+framed output stream, and the splitter sends one buffer per device call.
 Prints one JSON line per section, with the card's name and power limit.  --splitter-only runs section 2 alone."""
 from __future__ import annotations
 
@@ -35,6 +37,7 @@ WORKLOADS = {"rfc5424": (fb.FMT_RFC5424, 5424, 169.2), "rfc3164": (fb.FMT_RFC316
              "ltsv": (fb.FMT_LTSV, bench.SEEDS["ltsv"], bench.GEN_MEAN["ltsv"]),
              "gelf": (fb.FMT_GELF, bench.SEEDS["gelf"], bench.GEN_MEAN["gelf"])}
 RFC3164_YEAR = 2026
+OUT_FRAMINGS = {"none": fb.OUT_NONE, "line": fb.OUT_LINE, "nul": fb.OUT_NUL, "syslen": fb.OUT_SYSLEN}
 
 
 def card() -> dict:
@@ -92,6 +95,8 @@ def device_paths(args, stream: np.ndarray, soffs: np.ndarray, info: dict) -> Non
     split, pre = decoder(args.format, args.ltsv_typed, **cap), decoder(args.format, args.ltsv_typed, **cap)
     decode = decoder(args.format, args.ltsv_typed, **cap) if args.format != "rfc5424" else None
     try:
+        split.set_output_framing(OUT_FRAMINGS[args.out_framing])
+        pre.set_output_framing(OUT_FRAMINGS[args.out_framing])
         hs = split.host_alloc(len(stream))
         hs[:] = stream
         hl = pre.host_alloc(len(lines))
@@ -170,27 +175,37 @@ def splitter(args, stream: np.ndarray, info: dict) -> None:
         cuts.append(cuts[-1] + int(np.flatnonzero(stream[cuts[-1]:end] == ord("\n"))[-1]) + 1 if end < len(stream) else end)
     texts = [stream[a:b].tobytes() for a, b in zip(cuts[:-1], cuts[1:])]
     want = int(args.splitter_gb * 1e9)
+    framing = OUT_FRAMINGS[args.out_framing]
+    end = b"\0" if framing == fb.OUT_NUL else b"\n"  # one per record sent
+
+    def run(text):
+        if framing == fb.OUT_NONE:  # one record per send, the harness puts a "\n" after each
+            return fb.splitter_run_gelf(dec, text, max_lines=1 << 19, max_bytes=64 << 20)
+        return fb.splitter_run_gelf_framed(dec, text, framing, max_lines=1 << 19, max_bytes=64 << 20)[:2]
+
     dec = decoder(args.format, args.ltsv_typed, max_batch_bytes=64 << 20, max_batch_lines=1 << 20)
     wall, in_bytes, json_bytes, lines, n_rec, n_err = 0.0, 0, 0, 0, 0, 0
     try:
         small = texts[0][: 1 << 20]
-        fb.splitter_run_gelf(dec, small[: small.rindex(b"\n") + 1], max_lines=1 << 19, max_bytes=64 << 20)  # warm-up
+        run(small[: small.rindex(b"\n") + 1])  # warm-up
         k = 0
         while in_bytes < want:
             text = texts[k % len(texts)]
             k += 1
             t0 = time.perf_counter()
-            records, err = fb.splitter_run_gelf(dec, text, max_lines=1 << 19, max_bytes=64 << 20)
+            records, err = run(text)
             wall += time.perf_counter() - t0
-            r, e, t = records.count(b"\n"), err.count(b"\n"), text.count(b"\n")
+            r, e, t = records.count(end), err.count(b"\n"), text.count(b"\n")
+            sent = len(records) - (r if framing == fb.OUT_NONE else 0)
             assert r + e == t, (r, e, t)
             n_rec, n_err, lines = n_rec + r, n_err + e, lines + t
             in_bytes += len(text)
-            json_bytes += len(records) - r
+            json_bytes += sent
     finally:
         dec.close()
-    print(json.dumps({"section": "splitter", "api": "BatchingLineSplitter + CudaGelfEncoder (fgh_splitter_run_gelf: text in, "
-                      "records + stderr out, 64 MiB batches; wall time summed over calls of ~400 MB)", "calls": k,
+    print(json.dumps({"section": "splitter", "api": "BatchingLineSplitter + CudaGelfEncoder (fgh_splitter_run_gelf / "
+                      "fgh_splitter_run_gelf_framed: text in, records + stderr out, 64 MiB batches; wall time summed over calls "
+                      "of ~400 MB; json_bytes = the bytes sent, frames included)", "calls": k,
                       "lines": lines, "input_bytes": in_bytes, "json_bytes": json_bytes, "records": n_rec, "stderr_lines": n_err,
                       "wall_s": wall, "lines_per_s": lines / wall, "input_gb_per_s": in_bytes / wall / 1e9,
                       "output_gb_per_s": json_bytes / wall / 1e9, **info}), flush=True)
@@ -205,8 +220,10 @@ def main() -> None:
     ap.add_argument("--splitter-gb", type=float, default=1.0)
     ap.add_argument("--splitter-only", action="store_true")
     ap.add_argument("--ltsv-typed", action="store_true", help="ltsv: bench.py's schema and suffixes")
+    ap.add_argument("--out-framing", choices=sorted(OUT_FRAMINGS), default="none", help="output.framing, applied on the device")
     args = ap.parse_args()
     info = card()
+    info["out_framing"] = args.out_framing
     if args.format != "rfc5424":
         info["format"] = args.format
     if args.format == "ltsv":
