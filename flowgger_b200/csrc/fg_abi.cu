@@ -574,13 +574,17 @@ int launch_lines(fg_ctx* c, int fmt, int line0, int n, int tile, const uint8_t* 
 
 // The decoders whose device-resident results the fused GELF encoder reads.  LTSV only on a context created for it: the
 // pair keys carry that context's ltsv_suffixes.  GELF likewise, the rule LTSV follows.
-bool gelf_fusable(const fg_ctx* c, int fmt) {
-    return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || ((fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF) && c->input_format == fmt);
+int check_fusable(fg_ctx* c, int fmt) {
+    if (fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || ((fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF) && c->input_format == fmt))
+        return FG_OK;
+    return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
 }
 
+// Start of a fused GELF call: the LTSV stops and the wall clock of an earlier call end here, whatever this one returns.
 // gelf_decoder.rs:109 -> utils/mod.rs:16-21: the wall clock as secs + nanos / 1e9, read once at the start of a fused GELF
 // call for all its records without "timestamp"
-void begin_gelf_call(fg_ctx* c, int fmt) {
+void begin_fused(fg_ctx* c, int fmt) {
+    c->enc_stop_n = -1;
     c->gelf_now_ok = false;
     if (fmt != FG_FMT_GELF) return;
     timespec t;
@@ -1005,6 +1009,69 @@ int ensure_encoder(fg_ctx* c, int fmt, int chunks) {
     return FG_OK;
 }
 
+// After an overflow of a pipelined call: the allocators kept counting past the capacity, so each side table grows once to
+// the exact need, and the encoder's output buffer too when `enc_need` (its size in bytes, 0 without the encoder) passes it
+int regrow(fg_ctx* c, int fmt, const uint32_t* total, unsigned long long enc_need) {
+    if (int rc = regrow_tables(c, fmt, total)) return rc;
+    if (enc_need > c->enc_out_cap)
+        if (int rc = grow_enc_out(c, (size_t)enc_need + (size_t)enc_need / 8 + 4096)) return rc;
+    return FG_OK;
+}
+
+// End of a fused GELF call that encoded n records: its LTSV stops and wall clock become readable, and `out` points at
+// its results
+void end_fused(fg_ctx* c, int fmt, int32_t n, float kernel_ms, float total_ms, fg_encoded_out* out) {
+    if (fmt == FG_FMT_LTSV) c->enc_stop_n = n;
+    c->gelf_now_ok = fmt == FG_FMT_GELF;
+    memset(out, 0, sizeof *out);
+    out->n = n;
+    out->bytes = c->enc_out.h;
+    out->offsets = c->enc_offsets.h;
+    out->status = c->enc_status.h;
+    out->kernel_ms = kernel_ms;
+    out->total_ms = total_ms;
+}
+
+// The caller's lines, framed already -> H2D and the parse kernels chunk_lines lines a step, and with `encode` the GELF
+// encoder after each parse step: the pre-framed counterpart of split_stream, with the same results.  Without `encode`
+// the rows and side tables come back, with it only the encoded records.  total, kernel_ms, total_ms: as drain and finish
+// give them, zero for n == 0.
+int batch_lines(fg_ctx* c, int fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, bool encode, uint32_t* total,
+                float& kernel_ms, float& total_ms) {
+    if (int rc = begin_call(c, (fg_format)fmt)) return rc;
+    const int C = c->chunk_lines;
+    const int chunks = n > 0 ? (n + C - 1) / C : 1;
+    if (encode)
+        if (int rc = ensure_encoder(c, fmt, chunks)) return rc;
+    if (n == 0) {
+        if (encode) c->enc_offsets.h[0] = 0;
+        memset(total, 0, kCountBytes);
+        kernel_ms = total_ms = 0.f;
+        return FG_OK;
+    }
+    const auto t_begin = std::chrono::steady_clock::now();
+    HostBatch B{bytes, offsets, is_pinned(bytes), is_pinned(offsets), 0};
+    if (int rc = ensure_steps(c, chunks)) return rc;
+    const int tile = pick_tile(c, (size_t)(offsets[n] - offsets[0]), n, fmt);
+    const int attempts = encode ? 3 : 2;  // encode: a side table and the output buffer may each overflow once
+    for (int attempt = 0; attempt < attempts; ++attempt) {
+        FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, kCountBytes, c->s_comp));
+        if (encode) FG_CUDA(c, cudaMemsetAsync(c->enc_base.d, 0, sizeof(unsigned long long), c->s_comp));
+        B.bounce_ix = 0;
+        for (int k = 0; k < chunks; ++k) {
+            const int l0 = k * C, l1 = std::min(n, l0 + C);
+            if (int rc = upload_chunk(c, B, k, l0, l1)) return rc;
+            if (int rc = parse_step(c, fmt, k, l0, l1 - l0, tile, nullptr, 0, c->s_comp, encode)) return rc;
+        }
+        bool overflow;
+        if (int rc = drain(c, fmt, chunks, encode, total, overflow)) return rc;
+        if (int rc = finish(c, chunks, total, t_begin, kernel_ms, total_ms)) return rc;
+        if (!overflow) return FG_OK;
+        if (int rc = regrow(c, fmt, total, encode ? c->enc_base.h[chunks] : 0)) return rc;
+    }
+    return fail(c, FG_E_CAPACITY, encode ? "output / side table overflow after regrow" : "side table overflow after regrow");
+}
+
 // everything fg_create sets up on the device
 int init_device(fg_ctx* c, const fg_config* cfg) {
     FG_CUDA(c, cudaSetDevice(c->device));
@@ -1092,42 +1159,14 @@ int fg_decode_batch(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_
                     fg_batch_out* out) {
     if (!c || !out) return FG_E_ARG;
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
-    if (int rc = begin_call(c, fmt)) return rc;
+    uint32_t total[fg::K5_COUNT];
+    float kms, tms;
+    if (int rc = batch_lines(c, (int)fmt, bytes, offsets, n, false, total, kms, tms)) return rc;
     memset(out, 0, sizeof *out);
-    uint32_t total[fg::K5_COUNT] = {};
-    if (n == 0) {
-        fill_out(c, fmt, 0, total, out);
-        return FG_OK;
-    }
-    const auto t_begin = std::chrono::steady_clock::now();
-    HostBatch B{bytes, offsets, is_pinned(bytes), is_pinned(offsets), 0};
-    const int C = c->chunk_lines;
-    const int chunks = (n + C - 1) / C;
-    if (int rc = ensure_steps(c, chunks)) return rc;
-    const int tile = pick_tile(c, (size_t)(offsets[n] - offsets[0]), n, (int)fmt);
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, kCountBytes, c->s_comp));
-        B.bounce_ix = 0;
-        for (int k = 0; k < chunks; ++k) {
-            const int l0 = k * C, l1 = std::min(n, l0 + C);
-            if (int rc = upload_chunk(c, B, k, l0, l1)) return rc;
-            if (int rc = parse_step(c, fmt, k, l0, l1 - l0, tile, nullptr, 0, c->s_comp, false)) return rc;
-        }
-        bool overflow;
-        float kms, tms;
-        if (int rc = drain(c, fmt, chunks, false, total, overflow)) return rc;
-        if (int rc = finish(c, chunks, total, t_begin, kms, tms)) return rc;
-        if (overflow) {
-            // the allocators kept counting past the capacity: grow once to the exact need and redo
-            if (int rc = regrow_tables(c, fmt, total)) return rc;
-            continue;
-        }
-        fill_out(c, fmt, n, total, out);
-        out->kernel_ms = kms;
-        out->total_ms = tms;
-        return FG_OK;
-    }
-    return fail(c, FG_E_CAPACITY, "side table overflow after regrow");
+    fill_out(c, fmt, n, total, out);
+    out->kernel_ms = kms;
+    out->total_ms = tms;
+    return FG_OK;
 }
 
 int fg_set_rfc3164_year(fg_ctx* c, int32_t year) {
@@ -1223,58 +1262,14 @@ int fg_set_output_framing(fg_ctx* c, fg_out_framing framing) {
 // and side tables never leave the device.
 int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
     if (!c || !out) return FG_E_ARG;
-    c->enc_stop_n = -1;  // the stops of an earlier call end here, whatever this one returns
-    begin_gelf_call(c, (int)fmt);
+    begin_fused(c, (int)fmt);
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
-    if (!gelf_fusable(c, (int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
-    if (int rc = begin_call(c, fmt)) return rc;
-    const int C = c->chunk_lines;
-    const int chunks = n > 0 ? (n + C - 1) / C : 1;
-    if (int rc = ensure_encoder(c, (int)fmt, chunks)) return rc;
-    memset(out, 0, sizeof *out);
-    out->bytes = c->enc_out.h;
-    out->offsets = c->enc_offsets.h;
-    out->status = c->enc_status.h;
-    if (n == 0) {
-        c->enc_offsets.h[0] = 0;
-        if (fmt == FG_FMT_LTSV) c->enc_stop_n = 0;
-        c->gelf_now_ok = fmt == FG_FMT_GELF;
-        return FG_OK;
-    }
-    const auto t_begin = std::chrono::steady_clock::now();
-    HostBatch B{bytes, offsets, is_pinned(bytes), is_pinned(offsets), 0};
-    if (int rc = ensure_steps(c, chunks)) return rc;
-    const int tile = pick_tile(c, (size_t)(offsets[n] - offsets[0]), n, (int)fmt);
-    for (int attempt = 0; attempt < 3; ++attempt) {
-        FG_CUDA(c, cudaMemsetAsync(c->k.d, 0, kCountBytes, c->s_comp));
-        FG_CUDA(c, cudaMemsetAsync(c->enc_base.d, 0, sizeof(unsigned long long), c->s_comp));
-        B.bounce_ix = 0;
-        for (int k = 0; k < chunks; ++k) {
-            const int l0 = k * C, l1 = std::min(n, l0 + C);
-            if (int rc = upload_chunk(c, B, k, l0, l1)) return rc;
-            if (int rc = parse_step(c, fmt, k, l0, l1 - l0, tile, nullptr, 0, c->s_comp, true)) return rc;
-        }
-        uint32_t total[fg::K5_COUNT];
-        bool overflow;
-        float kms, tms;
-        if (int rc = drain(c, fmt, chunks, true, total, overflow)) return rc;
-        if (int rc = finish(c, chunks, total, t_begin, kms, tms)) return rc;
-        if (overflow) {
-            if (int rc = regrow_tables(c, fmt, total)) return rc;
-            const unsigned long long need = c->enc_base.h[chunks];
-            if (need > c->enc_out_cap)
-                if (int rc = grow_enc_out(c, (size_t)need + (size_t)need / 8 + 4096)) return rc;
-            out->bytes = c->enc_out.h;
-            continue;
-        }
-        out->n = n;
-        out->kernel_ms = kms;
-        out->total_ms = tms;
-        if (fmt == FG_FMT_LTSV) c->enc_stop_n = n;
-        c->gelf_now_ok = fmt == FG_FMT_GELF;
-        return FG_OK;
-    }
-    return fail(c, FG_E_CAPACITY, "output / side table overflow after regrow");
+    if (int rc = check_fusable(c, (int)fmt)) return rc;
+    uint32_t total[fg::K5_COUNT];
+    float kms, tms;
+    if (int rc = batch_lines(c, (int)fmt, bytes, offsets, n, true, total, kms, tms)) return rc;
+    end_fused(c, (int)fmt, n, kms, tms, out);
+    return FG_OK;
 }
 
 int fg_encoded_ltsv_stops(const fg_ctx* c, const int32_t** stop) {
@@ -1397,10 +1392,7 @@ int split_stream(fg_ctx* c, int fmt, fg_framing framing, const uint8_t* stream, 
             FG_CUDA(c, cudaMemcpyAsync(c->split_offsets.h, c->offsets.d, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, c->s_d2h));
         if (int rc = finish(c, nparse, total, t_begin, kernel_ms, total_ms)) return rc;
         if (overflow) {
-            if (int rc = regrow_tables(c, fmt, total)) return rc;
-            const unsigned long long need = encode ? c->enc_base.h[nparse] : 0;
-            if (need > c->enc_out_cap)
-                if (int rc = grow_enc_out(c, (size_t)need + (size_t)need / 8 + 4096)) return rc;
+            if (int rc = regrow(c, fmt, total, encode ? c->enc_base.h[nparse] : 0)) return rc;
             continue;
         }
         FG_CUDA(c, cudaEventElapsedTime(&c->last_split_ms, c->ev_s0, c->ev_s1));  // includes waiting for the H2D chunks
@@ -1438,22 +1430,13 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
 int fg_split_decode_encode_gelf(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
                                 const int32_t** line_offsets) {
     if (!c || !out || !line_offsets) return FG_E_ARG;
-    c->enc_stop_n = -1;  // the stops of an earlier call end here, whatever this one returns
-    begin_gelf_call(c, (int)fmt);
-    if (!gelf_fusable(c, (int)fmt)) return fail(c, FG_E_ARG, "the fused encoder takes input.format = rfc5424");
+    begin_fused(c, (int)fmt);
+    if (int rc = check_fusable(c, (int)fmt)) return rc;
     int32_t n;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;
     if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, true, n, total, kms, tms)) return rc;
-    if (fmt == FG_FMT_LTSV) c->enc_stop_n = n;
-    c->gelf_now_ok = fmt == FG_FMT_GELF;
-    memset(out, 0, sizeof *out);
-    out->n = n;
-    out->bytes = c->enc_out.h;
-    out->offsets = c->enc_offsets.h;
-    out->status = c->enc_status.h;
-    out->kernel_ms = kms;
-    out->total_ms = tms;
+    end_fused(c, (int)fmt, n, kms, tms, out);
     *line_offsets = c->split_offsets.h;
     return FG_OK;
 }

@@ -274,8 +274,8 @@ DecodeResult CudaBatchDecoder::materialize(const fg_batch_out& out, const uint8_
 }
 
 void CudaBatchDecoder::split_decode(const uint8_t* stream, int64_t nbytes, fg_batch_out* out, fg_framing framing) {
-    const int rc = fg_split_decode_framed(ctx_, fmt_, framing, stream, nbytes, out);
-    if (rc != FG_OK) throw std::runtime_error(std::string("fg_split_decode: ") + fg_last_error(ctx_));
+    if (!try_split_decode(stream, nbytes, out, framing))
+        throw std::runtime_error(std::string("fg_split_decode: ") + fg_last_error(ctx_));
 }
 
 bool CudaBatchDecoder::try_split_decode(const uint8_t* stream, int64_t nbytes, fg_batch_out* out, fg_framing framing) {
@@ -465,6 +465,16 @@ DecodeResult CudaBatchDecoder::materialize_line(const fg_batch_out& out, const u
     return materialize_record(fmt_, suffix_, out, bytes, line_lo, line_hi, i, side_effects);
 }
 
+// GELF without "timestamp": the reference stamps the record with the wall clock (gelf_decoder.rs:109 -> utils/mod.rs:16-21)
+static bool needs_wall_clock(const DecodeResult& r, const fg_batch_out& out, int32_t i) {
+    return r.ok() && (FG_META_FLAGS(row_meta(out, i)) & FG_FLAG_TS_MISSING);
+}
+static double wall_clock_ts() {
+    timespec tsn;
+    clock_gettime(CLOCK_REALTIME, &tsn);
+    return (double)tsn.tv_sec + (double)tsn.tv_nsec / 1e9;
+}
+
 // ---------------------------------------------------------------------------
 // Decoder trait objects
 // ---------------------------------------------------------------------------
@@ -483,49 +493,98 @@ DecodeResult CudaDecoder::decode(std::string_view line) const {
     std::vector<std::string> fx;
     DecodeResult r = impl_->materialize(out, bytes, offsets, 0, &fx);
     for (const auto& s : fx) fprintf(stdout, "%s\n", s.c_str());
-    if (r.ok() && (FG_META_FLAGS(row_meta(out, 0)) & FG_FLAG_TS_MISSING)) {
-        // gelf_decoder.rs:109 -> utils/mod.rs:16-21
-        timespec tsn;
-        clock_gettime(CLOCK_REALTIME, &tsn);
-        r.record.ts = (double)tsn.tv_sec + (double)tsn.tv_nsec / 1e9;
-    }
+    if (needs_wall_clock(r, out, 0)) r.record.ts = wall_clock_ts();
     return r;
 }
 std::unique_ptr<Decoder> CudaDecoder::clone_boxed() const { return std::unique_ptr<Decoder>(new CudaDecoder(impl_)); }
 
 // ---------------------------------------------------------------------------
-// RecordBatcher + the batching splitters
+// RecordEmitter, RecordBatcher + the batching splitters
 // ---------------------------------------------------------------------------
+namespace {
+
+constexpr const char* kInvalidUtf8 = "Invalid UTF-8 input";  // line_splitter.rs:23, nul_splitter.rs:25
+
+bool is_invalid_utf8_status(fg_format fmt, uint32_t status) {
+    const char* s = status ? fg_error_string(fmt, status) : nullptr;
+    return s && strcmp(s, kInvalidUtf8) == 0;
+}
+
+}  // namespace
+
+RecordEmitter::RecordEmitter(const Encoder& encoder, std::function<void(std::vector<uint8_t>&&)> tx, std::ostream& err_out,
+                             std::ostream& std_out, bool quiet_blank)
+    : encoder_(encoder), fused_(dynamic_cast<const CudaGelfEncoder*>(&encoder)), tx_(std::move(tx)), err_(err_out),
+      out_(std_out), quiet_blank_(quiet_blank) {}
+
+const CudaGelfEncoder* RecordEmitter::fused_with(const CudaBatchDecoder& gpu) const {
+    return fused_ != nullptr && CudaGelfEncoder::fuses_with(gpu.format()) ? fused_ : nullptr;
+}
+
+void RecordEmitter::emit(fg_format fmt, const fg_encoded_out& eo, const int32_t* stops, const uint8_t* bytes, int32_t i,
+                         int32_t lo, int32_t hi) {
+    if (stops && stops[i] >= 0) {
+        fx_.clear();
+        ltsv_missing_values(bytes, lo, hi, lo + stops[i], fx_);
+        for (const auto& s : fx_) out_ << s << "\n";
+    }
+    if (eo.status[i] != 0) reject(fmt, eo.status[i], fg_error_string(fmt, eo.status[i]), bytes, lo, hi);
+    else if (fused_->out_framing() == FG_OUT_NONE) tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
+}
+
+void RecordEmitter::end_batch(const fg_encoded_out& eo) {
+    if (fused_->out_framing() != FG_OUT_NONE && eo.offsets[eo.n] > 0) tx_(std::vector<uint8_t>(eo.bytes, eo.bytes + eo.offsets[eo.n]));
+}
+
+void RecordEmitter::emit(const CudaBatchDecoder& gpu, const fg_batch_out& out, const uint8_t* bytes, int32_t i, int32_t lo,
+                         int32_t hi) {
+    const fg_format fmt = gpu.format();
+    const uint32_t status = FG_META_STATUS(row_meta(out, i));
+    if (is_invalid_utf8_status(fmt, status)) {  // never decoded, so no side effects either
+        invalid_utf8();
+        return;
+    }
+    fx_.clear();
+    DecodeResult r = gpu.materialize_line(out, bytes, lo, hi, i, &fx_);
+    for (const auto& s : fx_) out_ << s << "\n";
+    const char* e = r.err;
+    if (!e) {
+        if (needs_wall_clock(r, out, i)) r.record.ts = wall_clock_ts();
+        std::vector<uint8_t> enc;
+        if (encoder_.encode(std::move(r.record), enc, &e)) {
+            tx_(std::move(enc));
+            return;
+        }
+    }
+    reject(fmt, status, e, bytes, lo, hi);
+}
+
+void RecordEmitter::invalid_utf8() { err_ << kInvalidUtf8 << "\n"; }
+
+// "Invalid UTF-8 input" for a record the device found not UTF-8, else "{err}: [{line.trim()}]"
+void RecordEmitter::reject(fg_format fmt, uint32_t status, const char* err, const uint8_t* bytes, int32_t lo, int32_t hi) {
+    if (is_invalid_utf8_status(fmt, status)) {
+        invalid_utf8();
+        return;
+    }
+    const std::string_view t = rust_trim(std::string_view((const char*)bytes + lo, (size_t)(hi - lo)));
+    if (quiet_blank_ && t.empty()) return;  // nul_splitter.rs:41-45
+    err_ << err << ": [" << t << "]\n";      // line_splitter.rs:37-39, nul_splitter.rs:43, syslen_splitter.rs:37
+}
+
 RecordBatcher::RecordBatcher(const Decoder& decoder, const Encoder& encoder, std::function<void(std::vector<uint8_t>&&)> tx,
                              std::ostream& err_out, std::ostream& std_out, Limits lim, bool quiet_blank)
-    : gpu_(decoder.batch()), encoder_(encoder), fused_(dynamic_cast<const CudaGelfEncoder*>(&encoder)), tx_(std::move(tx)),
-      err_(err_out), out_(std_out), quiet_blank_(quiet_blank) {
+    : gpu_(decoder.batch()), emit_(encoder, std::move(tx), err_out, std_out, quiet_blank) {
     // a batch never exceeds what the context can take (ADVICE r1: Limits used to be independent of DeviceOptions)
     max_bytes_ = std::min<int64_t>(lim.max_bytes, gpu_->capacity_bytes());
     max_lines_ = std::min<int32_t>(lim.max_lines, gpu_->capacity_lines());
     arena_.reserve((size_t)max_bytes_);
 }
 
-// "{err}: [{line.trim()}]" for a rejected record; `quiet_blank`: nothing for a blank one (the NUL splitter)
-static void report_error(std::ostream& err, const char* e, std::string_view line, bool quiet_blank) {
-    const std::string_view t = rust_trim(line);
-    if (quiet_blank && t.empty()) return;  // nul_splitter.rs:41-45
-    err << e << ": [" << t << "]\n";       // line_splitter.rs:37-39, nul_splitter.rs:43, syslen_splitter.rs:37
-}
-
-// GELF without "timestamp": the reference stamps the record with the wall clock (gelf_decoder.rs:109 -> utils/mod.rs:16-21)
-static double wall_clock_ts() {
-    timespec tsn;
-    clock_gettime(CLOCK_REALTIME, &tsn);
-    return (double)tsn.tv_sec + (double)tsn.tv_nsec / 1e9;
-}
-
-void RecordBatcher::report(const char* e, std::string_view line) { report_error(err_, e, line, quiet_blank_); }
-
 void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
     const int32_t n = (int32_t)offsets_.size() - 1;
     auto invalid = [&](int32_t i) {
-        for (int32_t k = 0; k < invalid_before_[(size_t)i]; ++k) err_ << "Invalid UTF-8 input\n";  // line_splitter.rs:22-25
+        for (int32_t k = 0; k < invalid_before_[(size_t)i]; ++k) emit_.invalid_utf8();
     };
     if (n == 0) {
         invalid(0);
@@ -535,47 +594,22 @@ void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
     const uint8_t dummy = 0;
     const uint8_t* bytes = arena_.empty() ? &dummy : arena_.data();
     std::lock_guard<std::mutex> guard(gpu->mutex());  // held until every Record of the batch has been materialised
-    if (fused_ != nullptr && CudaGelfEncoder::fuses_with(gpu->format())) {
+    if (const CudaGelfEncoder* fused = emit_.fused_with(*gpu)) {
         // decode + encode on the device (line_splitter.rs:50-52 fused): only the encoded records come back
         fg_encoded_out eo;
-        const bool framed = fused_->out_framing() != FG_OUT_NONE;  // one buffer for the batch: the Output's bytes
-        gpu->decode_encode_gelf(bytes, offsets_.data(), n, fused_->extra(), &eo, fused_->out_framing());
+        gpu->decode_encode_gelf(bytes, offsets_.data(), n, fused->extra(), &eo, fused->out_framing());
         const int32_t* stops = gpu->encoded_ltsv_stops();
-        std::vector<std::string> fx;
         for (int32_t i = 0; i < n; ++i) {
             invalid(i);
-            if (stops && stops[i] >= 0) {
-                fx.clear();
-                const int32_t lo = offsets_[(size_t)i];
-                ltsv_missing_values(bytes, lo, offsets_[(size_t)i + 1], lo + stops[i], fx);
-                for (const auto& s : fx) out_ << s << "\n";
-            }
-            if (eo.status[i] == 0) {
-                if (!framed) tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
-            } else {
-                report(fg_error_string(gpu->format(), eo.status[i]),
-                       std::string_view((const char*)bytes + offsets_[(size_t)i], (size_t)(offsets_[(size_t)i + 1] - offsets_[(size_t)i])));
-            }
+            emit_.emit(gpu->format(), eo, stops, bytes, i, offsets_[(size_t)i], offsets_[(size_t)i + 1]);
         }
-        if (framed && eo.offsets[n] > 0) tx_(std::vector<uint8_t>(eo.bytes, eo.bytes + eo.offsets[n]));
+        emit_.end_batch(eo);
     } else {
         fg_batch_out out;
         gpu->decode_batch(bytes, offsets_.data(), n, &out);
         for (int32_t i = 0; i < n; ++i) {
             invalid(i);
-            std::vector<std::string> fx;
-            DecodeResult r = gpu->materialize(out, bytes, offsets_.data(), i, &fx);
-            for (const auto& s : fx) out_ << s << "\n";
-            const char* e = r.err;
-            if (!e) {
-                if (FG_META_FLAGS(row_meta(out, i)) & FG_FLAG_TS_MISSING) r.record.ts = wall_clock_ts();
-                std::vector<uint8_t> enc;
-                if (encoder_.encode(std::move(r.record), enc, &e)) {
-                    tx_(std::move(enc));
-                    continue;
-                }
-            }
-            report(e, std::string_view((const char*)bytes + offsets_[(size_t)i], (size_t)(offsets_[(size_t)i + 1] - offsets_[(size_t)i])));
+            emit_.emit(*gpu, out, bytes, i, offsets_[(size_t)i], offsets_[(size_t)i + 1]);
         }
     }
     invalid(n);
@@ -604,13 +638,6 @@ void RecordBatcher::push(std::string_view line) {
 
 namespace {
 
-constexpr const char* kInvalidUtf8 = "Invalid UTF-8 input";  // line_splitter.rs:23, nul_splitter.rs:25
-
-bool is_invalid_utf8_status(fg_format fmt, uint32_t status) {
-    const char* s = status ? fg_error_string(fmt, status) : nullptr;
-    return s && strcmp(s, kInvalidUtf8) == 0;
-}
-
 // The line and NUL splitters: raw blocks of the stream, each cut after its last delimiter, are framed, checked for UTF-8
 // and decoded on the device (fg_split_decode_framed), with a CudaGelfEncoder on a decoder it fuses with also encoded there
 // (fg_split_decode_encode_gelf).  Records, stderr and stdout come out in stream order, exactly as the reference's
@@ -619,8 +646,8 @@ class BlockSplitter {
    public:
     BlockSplitter(fg_framing framing, bool quiet_blank, const Decoder& decoder, const Encoder& encoder,
                   const std::function<void(std::vector<uint8_t>&&)>& tx, std::ostream& err_out, std::ostream& std_out)
-        : framing_(framing), delim_(framing == FG_FRAME_NUL ? 0 : '\n'), quiet_blank_(quiet_blank), gpu_(decoder.batch()),
-          encoder_(encoder), fused_(dynamic_cast<const CudaGelfEncoder*>(&encoder)), tx_(tx), err_(err_out), out_(std_out) {}
+        : framing_(framing), delim_(framing == FG_FRAME_NUL ? 0 : '\n'), gpu_(decoder.batch()),
+          emit_(encoder, tx, err_out, std_out, quiet_blank) {}
 
     // blocks of up to `block_bytes` (at most the context's max_batch_bytes); a record longer than that grows its block
     void run(std::istream& in, int64_t block_bytes) {
@@ -674,75 +701,33 @@ class BlockSplitter {
     // false: more records than the context holds, nothing was emitted
     bool decode_on(CudaBatchDecoder* gpu, const uint8_t* p, int64_t n) {
         std::lock_guard<std::mutex> guard(gpu->mutex());  // held until every record of the block has been emitted
-        const fg_format fmt = gpu->format();
-        if (fused_ != nullptr && CudaGelfEncoder::fuses_with(fmt)) {
+        int32_t lo, hi;
+        if (const CudaGelfEncoder* fused = emit_.fused_with(*gpu)) {
             // framing + decode + encode on the device (line_splitter.rs:17-52 fused): only the encoded records come back
             fg_encoded_out eo;
             const int32_t* lines;
-            const bool framed = fused_->out_framing() != FG_OUT_NONE;  // one buffer for the block: the Output's bytes
-            if (!gpu->try_split_decode_encode_gelf(p, n, framing_, fused_->extra(), &eo, &lines, fused_->out_framing())) return false;
+            if (!gpu->try_split_decode_encode_gelf(p, n, framing_, fused->extra(), &eo, &lines, fused->out_framing())) return false;
             const int32_t* stops = gpu->encoded_ltsv_stops();
-            std::vector<std::string> fx;
             for (int32_t i = 0; i < eo.n; ++i) {
-                int32_t lo, hi;
                 split_extent(lines, p, i, lo, hi, framing_);
-                if (stops && stops[i] >= 0) {
-                    fx.clear();
-                    ltsv_missing_values(p, lo, hi, lines[i] + stops[i], fx);
-                    for (const auto& s : fx) out_ << s << "\n";
-                }
-                if (eo.status[i] == 0) {
-                    if (!framed) tx_(std::vector<uint8_t>(eo.bytes + eo.offsets[i], eo.bytes + eo.offsets[i + 1]));
-                    continue;
-                }
-                reject(fmt, eo.status[i], fg_error_string(fmt, eo.status[i]), p, lo, hi);
+                emit_.emit(gpu->format(), eo, stops, p, i, lo, hi);
             }
-            if (framed && eo.offsets[eo.n] > 0) tx_(std::vector<uint8_t>(eo.bytes, eo.bytes + eo.offsets[eo.n]));
+            emit_.end_batch(eo);
             return true;
         }
         fg_batch_out out;
         if (!gpu->try_split_decode(p, n, &out, framing_)) return false;
-        std::vector<std::string> fx;
         for (int32_t i = 0; i < out.n; ++i) {
-            int32_t lo, hi;
             split_extent(out.line_offsets, p, i, lo, hi, framing_);
-            const uint32_t meta = row_meta(out, i);
-            if (is_invalid_utf8_status(fmt, FG_META_STATUS(meta))) {
-                err_ << kInvalidUtf8 << "\n";
-                continue;
-            }
-            fx.clear();
-            DecodeResult r = gpu->materialize_line(out, p, lo, hi, i, &fx);
-            for (const auto& s : fx) out_ << s << "\n";
-            const char* e = r.err;
-            if (!e) {
-                if (FG_META_FLAGS(meta) & FG_FLAG_TS_MISSING) r.record.ts = wall_clock_ts();
-                std::vector<uint8_t> enc;
-                if (encoder_.encode(std::move(r.record), enc, &e)) {
-                    tx_(std::move(enc));
-                    continue;
-                }
-            }
-            reject(fmt, FG_META_STATUS(meta), e, p, lo, hi);
+            emit_.emit(*gpu, out, p, i, lo, hi);
         }
         return true;
     }
 
-    // "Invalid UTF-8 input" (line_splitter.rs:22-25), else "{err}: [{trim}]"
-    void reject(fg_format fmt, uint32_t status, const char* e, const uint8_t* p, int32_t lo, int32_t hi) {
-        if (is_invalid_utf8_status(fmt, status)) err_ << kInvalidUtf8 << "\n";
-        else report_error(err_, e, std::string_view((const char*)p + lo, (size_t)(hi - lo)), quiet_blank_);
-    }
-
     fg_framing framing_;
     uint8_t delim_;
-    bool quiet_blank_;
     std::shared_ptr<CudaBatchDecoder> gpu_;
-    const Encoder& encoder_;
-    const CudaGelfEncoder* fused_;
-    const std::function<void(std::vector<uint8_t>&&)>& tx_;
-    std::ostream& err_;
-    std::ostream& out_;
+    RecordEmitter emit_;
 };
 
 }  // namespace
@@ -955,6 +940,45 @@ void dump_result(const DecodeResult& r, bool ts_is_now, const std::vector<std::s
 // ---------------------------------------------------------------------------
 using namespace flowgger;
 
+namespace {
+
+// The canonical dumps of consecutive records: their text and each one's length
+struct Dumps {
+    std::string text;
+    std::vector<int64_t> lens;
+    void add(const DecodeResult& r, bool now, const std::vector<std::string>& side_effects) {
+        const size_t before = text.size();
+        dump_result(r, now, side_effects, text);
+        lens.push_back((int64_t)(text.size() - before));
+    }
+};
+
+// `parts` concatenated in order, handed out as one malloc'd buffer and int64 offsets [records + 1] (fgh_free both)
+int give_dumps(const Dumps* parts, size_t nparts, uint8_t** out_buf, int64_t** out_offsets) {
+    size_t bytes = 0, n = 0;
+    for (size_t t = 0; t < nparts; ++t) {
+        bytes += parts[t].text.size();
+        n += parts[t].lens.size();
+    }
+    uint8_t* buf = (uint8_t*)malloc(bytes ? bytes : 1);
+    int64_t* offs = (int64_t*)malloc(sizeof(int64_t) * (n + 1));
+    size_t pos = 0, li = 0;
+    offs[0] = 0;
+    for (size_t t = 0; t < nparts; ++t) {
+        memcpy(buf + pos, parts[t].text.data(), parts[t].text.size());
+        pos += parts[t].text.size();
+        for (const int64_t l : parts[t].lens) {
+            offs[li + 1] = offs[li] + l;
+            ++li;
+        }
+    }
+    *out_buf = buf;
+    *out_offsets = offs;
+    return 0;
+}
+
+}  // namespace
+
 extern "C" {
 
 void* fgh_decoder_new(int fmt, int device, int64_t max_bytes, int32_t max_lines, int32_t chunk_lines, int has_schema,
@@ -987,44 +1011,23 @@ int fgh_dump_range(void* d, const fg_batch_out* out, const uint8_t* bytes, const
     auto* dec = (CudaBatchDecoder*)d;
     const int64_t n = hi_line - lo_line;
     if (nthreads < 1) nthreads = 1;
-    std::vector<std::string> parts((size_t)nthreads);
-    std::vector<std::vector<int64_t>> lens((size_t)nthreads);
+    std::vector<Dumps> parts((size_t)nthreads);
     std::vector<std::thread> th;
     for (int t = 0; t < nthreads; ++t) {
         th.emplace_back([&, t] {
             const int64_t lo = lo_line + n * t / nthreads, hi = lo_line + n * (t + 1) / nthreads;
-            std::string& o = parts[(size_t)t];
-            lens[(size_t)t].reserve((size_t)(hi - lo));
+            Dumps& part = parts[(size_t)t];
+            part.lens.reserve((size_t)(hi - lo));
             std::vector<std::string> fx;
             for (int64_t i = lo; i < hi; ++i) {
-                const size_t before = o.size();
                 fx.clear();
                 DecodeResult r = dec->materialize(*out, bytes, offsets, (int32_t)i, &fx);
-                const bool now = r.ok() && (FG_META_FLAGS(row_meta(*out, (int32_t)i)) & FG_FLAG_TS_MISSING);
-                dump_result(r, now, fx, o);
-                lens[(size_t)t].push_back((int64_t)(o.size() - before));
+                part.add(r, needs_wall_clock(r, *out, (int32_t)i), fx);
             }
         });
     }
     for (auto& x : th) x.join();
-    size_t total = 0;
-    for (auto& p : parts) total += p.size();
-    uint8_t* buf = (uint8_t*)malloc(total ? total : 1);
-    int64_t* offs = (int64_t*)malloc(sizeof(int64_t) * (size_t)(n + 1));
-    size_t pos = 0;
-    int64_t li = 0;
-    offs[0] = 0;
-    for (int t = 0; t < nthreads; ++t) {
-        memcpy(buf + pos, parts[(size_t)t].data(), parts[(size_t)t].size());
-        for (const int64_t l : lens[(size_t)t]) {
-            offs[li + 1] = offs[li] + l;
-            ++li;
-        }
-        pos += parts[(size_t)t].size();
-    }
-    *out_buf = buf;
-    *out_offsets = offs;
-    return 0;
+    return give_dumps(parts.data(), parts.size(), out_buf, out_offsets);
 }
 int fgh_dump_out(void* d, const fg_batch_out* out, const uint8_t* bytes, const int32_t* offsets, int nthreads,
                  uint8_t** out_buf, int64_t** out_offsets) {
@@ -1035,26 +1038,17 @@ int fgh_dump_out(void* d, const fg_batch_out* out, const uint8_t* bytes, const i
 // over rows produced by the device-logic emulation (tests/emu)
 int fgh_dump_records(int fmt, const fg_batch_out* out, const uint8_t* bytes, const int32_t* offsets, const char* const* ltsv_suffix,
                      uint8_t** out_buf, int64_t** out_offsets) {
-    const int64_t n = out->n;
-    std::string all;
-    int64_t* offs = (int64_t*)malloc(sizeof(int64_t) * (size_t)(n + 1));
-    offs[0] = 0;
     std::string suffix[5];  // input.ltsv_suffixes by fg_ltsv_type (nullptr: none)
     for (int t = 1; t < 5 && ltsv_suffix; ++t)
         if (ltsv_suffix[t]) suffix[t] = ltsv_suffix[t];
+    Dumps dumps;
     std::vector<std::string> fx;
-    for (int64_t i = 0; i < n; ++i) {
+    for (int32_t i = 0; i < out->n; ++i) {
         fx.clear();
-        DecodeResult r = materialize_record((fg_format)fmt, suffix, *out, bytes, offsets[i], offsets[i + 1], (int32_t)i, &fx);
-        const bool now = r.ok() && (FG_META_FLAGS(row_meta(*out, (int32_t)i)) & FG_FLAG_TS_MISSING);
-        dump_result(r, now, fx, all);
-        offs[i + 1] = (int64_t)all.size();
+        DecodeResult r = materialize_record((fg_format)fmt, suffix, *out, bytes, offsets[i], offsets[i + 1], i, &fx);
+        dumps.add(r, needs_wall_clock(r, *out, i), fx);
     }
-    uint8_t* buf = (uint8_t*)malloc(all.size() ? all.size() : 1);
-    memcpy(buf, all.data(), all.size());
-    *out_buf = buf;
-    *out_offsets = offs;
-    return 0;
+    return give_dumps(&dumps, 1, out_buf, out_offsets);
 }
 
 // materialisation rate (owned Records, like the reference builds them), for the e2e report
@@ -1091,25 +1085,18 @@ int fgh_split_dump(void* d, int framing, const uint8_t* stream, int64_t nbytes, 
         fg_batch_out out;
         dec->split_decode(stream, nbytes, &out, (fg_framing)framing);
         const int32_t n = out.n;
-        std::string all;
-        int64_t* offs = (int64_t*)malloc(sizeof(int64_t) * ((size_t)n + 1));
-        int32_t* lo_out = (int32_t*)malloc(sizeof(int32_t) * ((size_t)n + 1));
-        offs[0] = 0;
+        Dumps dumps;
         std::vector<std::string> fx;
         for (int32_t i = 0; i < n; ++i) {
             int32_t lo, hi;
             split_extent(out.line_offsets, stream, i, lo, hi, (fg_framing)framing);
             fx.clear();
             DecodeResult r = dec->materialize_line(out, stream, lo, hi, i, &fx);
-            const bool now = r.ok() && (FG_META_FLAGS(row_meta(out, i)) & FG_FLAG_TS_MISSING);
-            dump_result(r, now, fx, all);
-            offs[i + 1] = (int64_t)all.size();
+            dumps.add(r, needs_wall_clock(r, out, i), fx);
         }
+        int32_t* lo_out = (int32_t*)malloc(sizeof(int32_t) * ((size_t)n + 1));
         memcpy(lo_out, out.line_offsets, sizeof(int32_t) * ((size_t)n + 1));
-        uint8_t* buf = (uint8_t*)malloc(all.size() ? all.size() : 1);
-        memcpy(buf, all.data(), all.size());
-        *out_buf = buf;
-        *out_offsets = offs;
+        give_dumps(&dumps, 1, out_buf, out_offsets);
         *out_line_offsets = lo_out;
         *out_n = n;
         if (kernel_ms) *kernel_ms = out.kernel_ms;
@@ -1133,7 +1120,7 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
         CudaDecoder root((fg_format)fmt, {}, opt);
         std::vector<std::unique_ptr<Decoder>> clones;
         for (int t = 0; t < nthreads; ++t) clones.push_back(root.clone_boxed());
-        std::vector<std::string> dumps((size_t)n);
+        std::vector<DecodeResult> results((size_t)n);
         std::vector<std::thread> th;
         std::vector<std::string> errs((size_t)nthreads);
         for (int t = 0; t < nthreads; ++t) {
@@ -1141,8 +1128,7 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
                 try {
                     for (int32_t i = t; i < n; i += nthreads) {
                         std::string_view line((const char*)bytes + offsets[i], (size_t)(offsets[i + 1] - offsets[i]));
-                        DecodeResult r = clones[(size_t)t]->decode(line);
-                        dump_result(r, false, {}, dumps[(size_t)i]);
+                        results[(size_t)i] = clones[(size_t)t]->decode(line);
                     }
                 } catch (const std::exception& e) {
                     errs[(size_t)t] = e.what();
@@ -1152,18 +1138,9 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
         for (auto& x : th) x.join();
         for (const auto& e : errs)
             if (!e.empty()) throw std::runtime_error(e);
-        std::string all;
-        int64_t* offs = (int64_t*)malloc(sizeof(int64_t) * ((size_t)n + 1));
-        offs[0] = 0;
-        for (int32_t i = 0; i < n; ++i) {
-            all += dumps[(size_t)i];
-            offs[i + 1] = (int64_t)all.size();
-        }
-        uint8_t* buf = (uint8_t*)malloc(all.size() ? all.size() : 1);
-        memcpy(buf, all.data(), all.size());
-        *out_buf = buf;
-        *out_offsets = offs;
-        return 0;
+        Dumps dumps;
+        for (const DecodeResult& r : results) dumps.add(r, false, {});
+        return give_dumps(&dumps, 1, out_buf, out_offsets);
     } catch (const std::exception& e) {
         if (errbuf && errlen > 0) snprintf(errbuf, (size_t)errlen, "%s", e.what());
         return -1;
@@ -1174,11 +1151,10 @@ int fgh_clone_decode_threads(int fmt, int device, const uint8_t* bytes, const in
 
 namespace {
 
-// The harness of the two gelf splitter entries: BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or
+// The harness of the splitter entries: BatchingLineSplitter (framing 0), BatchingNulSplitter (framing 1) or
 // BatchingSyslenSplitter (framing 2, through RecordBatcher) over `text` with `enc`; `tx` receives what the splitter sends
-int run_gelf_splitter(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int framing,
-                      const CudaGelfEncoder& enc, const std::function<void(std::vector<uint8_t>&&)>& tx, std::string& err,
-                      std::string& out) {
+int run_splitter(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int framing, const Encoder& enc,
+                 const std::function<void(std::vector<uint8_t>&&)>& tx, std::string& err, std::string& out) {
     struct Shared : Decoder {
         std::shared_ptr<CudaBatchDecoder> b;
         DecodeResult decode(std::string_view) const override { return {}; }
@@ -1195,7 +1171,7 @@ int run_gelf_splitter(void* d, const uint8_t* text, int64_t len, int32_t max_lin
     try {
         if (framing == 1) BatchingNulSplitter(lim).run(is, tx, dec, enc, es, os);        // input.framing = "nul"
         else if (framing == 2) BatchingSyslenSplitter(lim).run(is, tx, dec, enc, es, os);  // input.framing = "syslen"
-        else BatchingLineSplitter(lim).run(is, tx, dec, enc, es, os);
+        else BatchingLineSplitter(lim).run(is, tx, dec, enc, es, os);                      // input.framing = "line"
     } catch (const std::exception&) {
         return -1;
     }
@@ -1228,7 +1204,7 @@ int fgh_splitter_run_gelf(void* d, const uint8_t* text, int64_t len, int32_t max
                           uint8_t** out_stderr, int64_t* out_stderr_len, int framing, uint8_t** out_stdout, int64_t* out_stdout_len) {
     std::string records, err, out;
     auto tx = [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); };
-    if (run_gelf_splitter(d, text, len, max_lines, max_bytes, framing, CudaGelfEncoder(extra_of(n_extra, keys, vals)), tx, err, out))
+    if (run_splitter(d, text, len, max_lines, max_bytes, framing, CudaGelfEncoder(extra_of(n_extra, keys, vals)), tx, err, out))
         return -1;
     give(records, out_records, out_records_len);
     give(err, out_stderr, out_stderr_len);
@@ -1245,7 +1221,7 @@ int fgh_splitter_run_gelf_framed(void* d, const uint8_t* text, int64_t len, int3
     std::string stream, err, out;
     auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
     const CudaGelfEncoder enc(extra_of(n_extra, keys, vals), (fg_out_framing)out_framing);
-    if (run_gelf_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
+    if (run_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
     give(stream, out_stream, out_stream_len);
     give(err, out_stderr, out_stderr_len);
     give(out, out_stdout, out_stdout_len);
@@ -1266,25 +1242,16 @@ int fgh_multi_decode_dump(int fmt, const int* devices, int ndev, int64_t max_byt
         opt.max_batch_lines = max_lines;
         MultiGpuBatchDecoder dec((fg_format)fmt, std::vector<int>(devices, devices + ndev), {}, opt);
         const auto& shards = dec.decode_batch(bytes, offsets, n);
-        std::string all;
-        int64_t* offs = (int64_t*)malloc(sizeof(int64_t) * ((size_t)n + 1));
-        offs[0] = 0;
+        Dumps dumps;
         std::vector<std::string> fx;
         size_t g = 0;
         for (int32_t i = 0; i < n; ++i) {
             fx.clear();
             DecodeResult r = dec.materialize(i, bytes, &fx);
             while (g + 1 < shards.size() && i >= shards[g].line0 + shards[g].n) ++g;  // the shard that holds line i
-            // GELF without a timestamp: the reference stamps the record with the wall clock (gelf_decoder.rs:109)
-            const bool now = r.ok() && (FG_META_FLAGS(row_meta(shards[g].out, i - shards[g].line0)) & FG_FLAG_TS_MISSING);
-            dump_result(r, now, fx, all);
-            offs[i + 1] = (int64_t)all.size();
+            dumps.add(r, needs_wall_clock(r, shards[g].out, i - shards[g].line0), fx);
         }
-        uint8_t* buf = (uint8_t*)malloc(all.size() ? all.size() : 1);
-        memcpy(buf, all.data(), all.size());
-        *out_buf = buf;
-        *out_offsets = offs;
-        return 0;
+        return give_dumps(&dumps, 1, out_buf, out_offsets);
     } catch (const std::exception& e) {
         if (errbuf && errlen > 0) snprintf(errbuf, (size_t)errlen, "%s", e.what());
         return -1;
@@ -1306,37 +1273,12 @@ int fgh_splitter_run(void* d, int framing, const uint8_t* text, int64_t len, int
             return true;
         }
     };
-    struct Shared : Decoder {
-        std::shared_ptr<CudaBatchDecoder> b;
-        DecodeResult decode(std::string_view) const override { return {}; }
-        std::unique_ptr<Decoder> clone_boxed() const override { return nullptr; }
-        std::shared_ptr<CudaBatchDecoder> batch() const override { return b; }
-    } dec;
-    dec.b = std::shared_ptr<CudaBatchDecoder>((CudaBatchDecoder*)d, [](CudaBatchDecoder*) {});
-    BatchingLineSplitter::Limits lim;
-    lim.max_lines = max_lines;
-    lim.max_bytes = max_bytes;
-    std::string in((const char*)text, (size_t)len);
-    std::istringstream is(in);
-    std::ostringstream es, os;
-    std::string records;
-    DumpEncoder enc;
-    try {
-        auto tx = [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); };
-        if (framing == 1) BatchingNulSplitter(lim).run(is, tx, dec, enc, es, os);        // input.framing = "nul"
-        else if (framing == 2) BatchingSyslenSplitter(lim).run(is, tx, dec, enc, es, os);  // input.framing = "syslen"
-        else BatchingLineSplitter(lim).run(is, tx, dec, enc, es, os);                      // input.framing = "line"
-    } catch (const std::exception&) {
-        return -1;
-    }
-    auto give = [](const std::string& s, uint8_t** p, int64_t* n) {
-        *p = (uint8_t*)malloc(s.size() ? s.size() : 1);
-        memcpy(*p, s.data(), s.size());
-        *n = (int64_t)s.size();
-    };
+    std::string records, err, out;
+    auto tx = [&](std::vector<uint8_t>&& v) { records.append(v.begin(), v.end()); records.push_back('\n'); };
+    if (run_splitter(d, text, len, max_lines, max_bytes, framing, DumpEncoder(), tx, err, out)) return -1;
     give(records, out_records, out_records_len);
-    give(es.str(), out_stderr, out_stderr_len);
-    give(os.str(), out_stdout, out_stdout_len);
+    give(err, out_stderr, out_stderr_len);
+    give(out, out_stdout, out_stdout_len);
     return 0;
 }
 

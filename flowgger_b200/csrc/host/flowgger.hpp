@@ -211,13 +211,43 @@ class CudaGelfEncoder : public Encoder {
     fg_out_framing out_framing_;
 };
 
+// What RecordBatcher and the batching splitters do with each record of a batch decoded on the device, one record at a
+// time in stream order, as the reference's per-record call sites do: LTSV's "Missing value" lines on stdout
+// (ltsv_decoder.rs:99), then the encoded record to `tx`, or "{err}: [{line.trim()}]" / "Invalid UTF-8 input" on stderr.
+// The caller gives record i's extent [lo, hi) in its bytes, without the terminator.
+class RecordEmitter {
+   public:
+    RecordEmitter(const Encoder& encoder, std::function<void(std::vector<uint8_t>&&)> tx, std::ostream& err_out,
+                  std::ostream& std_out, bool quiet_blank);
+    // the encoder when it runs fused with the decoder of `gpu` (CudaGelfEncoder::fuses_with), else nullptr
+    const CudaGelfEncoder* fused_with(const CudaBatchDecoder& gpu) const;
+    // record i of a fused call on a decoder of format `fmt`; `stops` = CudaBatchDecoder::encoded_ltsv_stops()
+    void emit(fg_format fmt, const fg_encoded_out& eo, const int32_t* stops, const uint8_t* bytes, int32_t i, int32_t lo,
+              int32_t hi);
+    // record i of a batch `gpu` decoded: materialised and encoded on the host
+    void emit(const CudaBatchDecoder& gpu, const fg_batch_out& out, const uint8_t* bytes, int32_t i, int32_t lo, int32_t hi);
+    // after the records of a fused call: with output.framing, the framed records of the whole call in one `tx`
+    void end_batch(const fg_encoded_out& eo);
+    // "Invalid UTF-8 input" on stderr (line_splitter.rs:22-25, nul_splitter.rs:25)
+    void invalid_utf8();
+
+   private:
+    void reject(fg_format fmt, uint32_t status, const char* err, const uint8_t* bytes, int32_t lo, int32_t hi);
+    const Encoder& encoder_;
+    const CudaGelfEncoder* fused_;
+    std::function<void(std::vector<uint8_t>&&)> tx_;
+    std::ostream& err_;
+    std::ostream& out_;
+    bool quiet_blank_;  // nothing on stderr for a blank rejected record (the NUL splitter)
+    std::vector<std::string> fx_;  // side effects of the record in hand
+};
+
 // The batching twin of the reference's per-record call sites (`decode -> encode -> tx.send`, or print
 // "{err}: [{line.trim()}]" to stderr): line_splitter.rs:50, nul_splitter.rs:57, syslen_splitter.rs:65,
 // input/udp_input.rs:139, input/redis_input.rs:159, input/file/worker.rs:116.  A caller frames its records as the old
 // code did and push()es each one; the batcher accumulates up to Limits, decodes the batch on the GPU in one call and then,
 // in the original order, encodes + sends every Record or prints the identical stderr line.  With a CudaGelfEncoder and a
 // decoder it fuses with (CudaGelfEncoder::fuses_with) the two stages run fused on the device (fg_decode_encode_gelf).
-class CudaGelfEncoder;
 class RecordBatcher {
    public:
     struct Limits {
@@ -232,14 +262,8 @@ class RecordBatcher {
 
    private:
     void flush_on(CudaBatchDecoder* gpu);
-    void report(const char* err, std::string_view line);
     std::shared_ptr<CudaBatchDecoder> gpu_;
-    const Encoder& encoder_;
-    const CudaGelfEncoder* fused_;
-    std::function<void(std::vector<uint8_t>&&)> tx_;
-    std::ostream& err_;
-    std::ostream& out_;
-    bool quiet_blank_;
+    RecordEmitter emit_;
     int64_t max_bytes_;
     int32_t max_lines_;
     std::vector<uint8_t> arena_;

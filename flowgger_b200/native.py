@@ -198,6 +198,53 @@ def _ptr(a: np.ndarray) -> C.c_void_p:
     return C.c_void_p(a.ctypes.data)
 
 
+def _c_strings(xs: list[str]):
+    return (C.c_char_p * max(len(xs), 1))(*[x.encode() for x in xs])
+
+
+def _extra_arrays(extra: dict[str, str] | None):
+    """output.gelf_extra as (count, keys, values) C string arrays."""
+    ex = list((extra or {}).items())
+    return len(ex), _c_strings([k for k, _ in ex]), _c_strings([v for _, v in ex])
+
+
+def _take_dumps(pb: C.c_void_p, po: C.c_void_p, n: int) -> tuple[bytes, np.ndarray]:
+    """Reads and frees the (buffer, int64 offsets[n + 1]) pair of canonical dumps an fgh_* entry returned."""
+    H = load_host()
+    try:
+        offs = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_int64)), shape=(n + 1,)).copy()
+        buf = C.string_at(pb, int(offs[-1]))
+    finally:
+        H.fgh_free(pb)
+        H.fgh_free(po)
+    return buf, offs
+
+
+def _encoded_views(out: FgEncodedOut):
+    """Views of an fg_encoded_out: (JSON bytes, int64 offsets[n + 1], status uint8[n])."""
+    n = out.n
+    offs = np.ctypeslib.as_array(out.offsets, shape=(n + 1,))
+    total = int(offs[-1]) if n else 0
+    buf = np.ctypeslib.as_array(out.bytes, shape=(max(total, 1),))[:total]
+    status = np.ctypeslib.as_array(out.status, shape=(max(n, 1),))[:n]
+    return buf, offs, status
+
+
+def _run_splitter(call) -> tuple[bytes, bytes, bytes]:
+    """Runs a splitter entry with three malloc'd (pointer, length) outputs, `call(outs)` given their six by-reference
+    arguments in order, and returns and frees the outputs."""
+    H = load_host()
+    ps = [C.c_void_p() for _ in range(3)]
+    ns = [C.c_int64() for _ in range(3)]
+    if call([a for p, n in zip(ps, ns) for a in (C.byref(p), C.byref(n))]) != 0:
+        raise RuntimeError("splitter failed")
+    out = []
+    for p, n in zip(ps, ns):
+        out.append(C.string_at(p, n.value))
+        H.fgh_free(p)
+    return tuple(out)
+
+
 class BatchResult:
     """numpy views over one fg_batch_out (valid until the next decode on the same decoder)."""
 
@@ -280,18 +327,11 @@ class BatchDecoder:
         self.fmt = fmt
         schema = list((ltsv_schema or {}).items())
         suff = list((ltsv_suffixes or {}).items())
-
-        def carr(xs):
-            a = (C.c_char_p * max(len(xs), 1))()
-            for i, x in enumerate(xs):
-                a[i] = x.encode()
-            return a
-
         err = C.create_string_buffer(512)
         h = self.H.fgh_decoder_new(fmt, device, max_batch_bytes, max_batch_lines, chunk_lines,
                                    1 if ltsv_schema is not None else 0, len(schema),
-                                   carr([k for k, _ in schema]), carr([v for _, v in schema]), len(suff),
-                                   carr([k for k, _ in suff]), carr([v for _, v in suff]), err, 512)
+                                   _c_strings([k for k, _ in schema]), _c_strings([v for _, v in schema]), len(suff),
+                                   _c_strings([k for k, _ in suff]), _c_strings([v for _, v in suff]), err, 512)
         if not h:
             raise RuntimeError(err.value.decode() or "fgh_decoder_new failed")
         self._h = C.c_void_p(h)
@@ -356,10 +396,7 @@ class BatchDecoder:
 
     def set_gelf_extra(self, extra: dict[str, str]) -> None:
         """output.gelf_extra of GelfEncoder::new (gelf_encoder.rs:29-48)."""
-        ex = list(extra.items())
-        keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])
-        vals = (C.c_char_p * max(len(ex), 1))(*[v.encode() for _, v in ex])
-        self._check(self.L.fg_set_gelf_extra(self.ctx, len(ex), keys, vals), "fg_set_gelf_extra")
+        self._check(self.L.fg_set_gelf_extra(self.ctx, *_extra_arrays(extra)), "fg_set_gelf_extra")
 
     def set_output_framing(self, framing: int) -> None:
         """output.framing of the fused calls (fg_set_output_framing): OUT_NONE, OUT_LINE ("\\n" after each record), OUT_NUL
@@ -384,10 +421,7 @@ class BatchDecoder:
         self._keep = (data, offsets)
         self._check(self.L.fg_decode_encode_gelf(self.ctx, self.fmt, _ptr(data), _ptr(offsets), n, C.byref(out)), "fg_decode_encode_gelf")
         self._last_encoded_n = n
-        offs = np.ctypeslib.as_array(out.offsets, shape=(n + 1,))
-        total = int(offs[-1]) if n else 0
-        buf = np.ctypeslib.as_array(out.bytes, shape=(max(total, 1),))[:total]
-        status = np.ctypeslib.as_array(out.status, shape=(max(n, 1),))[:n]
+        buf, offs, status = _encoded_views(out)
         if copy:
             return buf.tobytes(), offs.copy(), status.copy(), out.kernel_ms
         return buf, offs, status, out.kernel_ms
@@ -406,10 +440,7 @@ class BatchDecoder:
                     "fg_split_decode_encode_gelf")
         n = out.n
         self._last_encoded_n = n
-        offs = np.ctypeslib.as_array(out.offsets, shape=(n + 1,))
-        total = int(offs[-1]) if n else 0
-        buf = np.ctypeslib.as_array(out.bytes, shape=(max(total, 1),))[:total]
-        status = np.ctypeslib.as_array(out.status, shape=(max(n, 1),))[:n]
+        buf, offs, status = _encoded_views(out)
         lines = np.ctypeslib.as_array(lo, shape=(n + 1,))
         if copy:
             return buf.tobytes(), offs.copy(), status.copy(), lines.copy(), out.kernel_ms
@@ -478,13 +509,7 @@ class BatchDecoder:
         hi = res.n if hi is None else hi
         pb, po = C.c_void_p(), C.c_void_p()
         self.H.fgh_dump_range(self._h, C.byref(res.raw), _ptr(data), _ptr(offsets), lo, hi, nthreads, C.byref(pb), C.byref(po))
-        try:
-            offs = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_int64)), shape=(hi - lo + 1,)).copy()
-            buf = C.string_at(pb, int(offs[-1]))
-        finally:
-            self.H.fgh_free(pb)
-            self.H.fgh_free(po)
-        return buf, offs
+        return _take_dumps(pb, po, hi - lo)
 
     def split_dump(self, stream: np.ndarray, framing: int = 0) -> tuple[bytes, np.ndarray, np.ndarray, float]:
         """fg_split_decode_framed on a raw byte stream (framing 0 = "line", 1 = "nul"): (canonical dumps, dump offsets,
@@ -497,14 +522,10 @@ class BatchDecoder:
         if rc != 0:
             raise RuntimeError(err.value.decode())
         try:
-            offs = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_int64)), shape=(n.value + 1,)).copy()
             lines = np.ctypeslib.as_array(C.cast(pl, C.POINTER(C.c_int32)), shape=(n.value + 1,)).copy()
-            buf = C.string_at(pb, int(offs[-1]))
         finally:
-            self.H.fgh_free(pb)
-            self.H.fgh_free(po)
             self.H.fgh_free(pl)
-        return buf, offs, lines, ms.value
+        return *_take_dumps(pb, po, n.value), lines, ms.value
 
     def materialize_seconds(self, res: BatchResult, data: np.ndarray, offsets: np.ndarray, nthreads: int = 1) -> float:
         return float(self.H.fgh_materialize_bench(self._h, C.byref(res.raw), _ptr(data), _ptr(offsets), nthreads))
@@ -520,13 +541,7 @@ def dump_records(fmt: int, out: FgBatchOut, data: np.ndarray, offsets: np.ndarra
     if ltsv_suffix is not None:
         suf = (C.c_char_p * 5)(*[s if s is None else bytes(s) for s in ltsv_suffix])
     H.fgh_dump_records(fmt, C.byref(out), _ptr(data), _ptr(offsets), suf, C.byref(pb), C.byref(po))
-    try:
-        offs = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_int64)), shape=(out.n + 1,)).copy()
-        buf = C.string_at(pb, int(offs[-1]))
-    finally:
-        H.fgh_free(pb)
-        H.fgh_free(po)
-    return buf, offs
+    return _take_dumps(pb, po, out.n)
 
 
 def tz_lookup(name: str, local: int, tzdir: str | None = None):
@@ -562,13 +577,7 @@ def multi_gpu_decode_dump(fmt: int, devices: list[int], data: np.ndarray, offset
                                  C.byref(pb), C.byref(po), err, 512)
     if rc != 0:
         raise RuntimeError(err.value.decode())
-    try:
-        offs = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_int64)), shape=(n + 1,)).copy()
-        buf = C.string_at(pb, int(offs[-1]))
-    finally:
-        H.fgh_free(pb)
-        H.fgh_free(po)
-    return buf, offs
+    return _take_dumps(pb, po, n)
 
 
 def clone_decode_threads(fmt: int, lines: list[bytes], nthreads: int = 2, device: int = 0) -> list[bytes]:
@@ -582,12 +591,7 @@ def clone_decode_threads(fmt: int, lines: list[bytes], nthreads: int = 2, device
     rc = H.fgh_clone_decode_threads(fmt, device, _ptr(data), _ptr(offs), len(lines), nthreads, C.byref(pb), C.byref(po), err, 512)
     if rc != 0:
         raise RuntimeError(err.value.decode())
-    try:
-        o = np.ctypeslib.as_array(C.cast(po, C.POINTER(C.c_int64)), shape=(len(lines) + 1,)).copy()
-        buf = C.string_at(pb, int(o[-1]))
-    finally:
-        H.fgh_free(pb)
-        H.fgh_free(po)
+    buf, o = _take_dumps(pb, po, len(lines))
     return [buf[o[i]:o[i + 1]] for i in range(len(lines))]
 
 
@@ -598,20 +602,10 @@ def splitter_run_gelf(dec: "BatchDecoder", text: bytes, extra: dict[str, str] | 
     and output.format = gelf (decode and encode fused on the GPU, framing too for 0 and 1): returns (JSON records
     separated by newlines, stderr text), and with stdout=True also the stdout text (LTSV's "Missing value" lines)."""
     H = load_host()
-    ex = list((extra or {}).items())
-    keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])
-    vals = (C.c_char_p * max(len(ex), 1))(*[v.encode() for _, v in ex])
-    ps = [C.c_void_p() for _ in range(3)]
-    ns = [C.c_int64() for _ in range(3)]
-    rc = H.fgh_splitter_run_gelf(dec._h, text, len(text), max_lines, max_bytes, len(ex), keys, vals, C.byref(ps[0]), C.byref(ns[0]),
-                                 C.byref(ps[1]), C.byref(ns[1]), framing, C.byref(ps[2]), C.byref(ns[2]))
-    if rc != 0:
-        raise RuntimeError("splitter failed")
-    out = []
-    for p, n in zip(ps, ns):
-        out.append(C.string_at(p, n.value))
-        H.fgh_free(p)
-    return tuple(out) if stdout else tuple(out[:2])
+    n_extra, keys, vals = _extra_arrays(extra)
+    out = _run_splitter(lambda o: H.fgh_splitter_run_gelf(dec._h, text, len(text), max_lines, max_bytes, n_extra, keys, vals,
+                                                          *o[:4], framing, *o[4:]))
+    return out if stdout else out[:2]
 
 
 def splitter_run_gelf_framed(dec: "BatchDecoder", text: bytes, out_framing: int, extra: dict[str, str] | None = None,
@@ -619,22 +613,9 @@ def splitter_run_gelf_framed(dec: "BatchDecoder", text: bytes, out_framing: int,
     """splitter_run_gelf with output.framing applied on the device (OUT_NONE, OUT_LINE, OUT_NUL or OUT_SYSLEN): returns
     (the output stream exactly as the splitter sent it, stderr text, stdout text)."""
     H = load_host()
-    ex = list((extra or {}).items())
-    keys = (C.c_char_p * max(len(ex), 1))(*[k.encode() for k, _ in ex])
-    vals = (C.c_char_p * max(len(ex), 1))(*[v.encode() for _, v in ex])
-    ps = [C.c_void_p() for _ in range(3)]
-    ns = [C.c_int64() for _ in range(3)]
-    args = []
-    for p, n in zip(ps, ns):
-        args += [C.byref(p), C.byref(n)]
-    rc = H.fgh_splitter_run_gelf_framed(dec._h, text, len(text), max_lines, max_bytes, len(ex), keys, vals, framing, out_framing, *args)
-    if rc != 0:
-        raise RuntimeError("splitter failed")
-    out = []
-    for p, n in zip(ps, ns):
-        out.append(C.string_at(p, n.value))
-        H.fgh_free(p)
-    return tuple(out)
+    n_extra, keys, vals = _extra_arrays(extra)
+    return _run_splitter(lambda o: H.fgh_splitter_run_gelf_framed(dec._h, text, len(text), max_lines, max_bytes, n_extra, keys,
+                                                                  vals, framing, out_framing, *o))
 
 
 def splitter_run(dec: "BatchDecoder", text: bytes, max_lines: int = 1 << 16, max_bytes: int = 16 << 20,
@@ -642,16 +623,4 @@ def splitter_run(dec: "BatchDecoder", text: bytes, max_lines: int = 1 << 16, max
     """Batching splitter over `text` (the stdin of config #1); framing 0 = "line", 1 = "nul", 2 = "syslen" (input.framing):
     returns (records, stderr, stdout)."""
     H = load_host()
-    ps = [C.c_void_p() for _ in range(3)]
-    ns = [C.c_int64() for _ in range(3)]
-    args = []
-    for p, n in zip(ps, ns):
-        args += [C.byref(p), C.byref(n)]
-    rc = H.fgh_splitter_run(dec._h, framing, text, len(text), max_lines, max_bytes, *args)
-    if rc != 0:
-        raise RuntimeError("splitter failed")
-    out = []
-    for p, n in zip(ps, ns):
-        out.append(C.string_at(p, n.value))
-        H.fgh_free(p)
-    return tuple(out)
+    return _run_splitter(lambda o: H.fgh_splitter_run(dec._h, framing, text, len(text), max_lines, max_bytes, *o))
