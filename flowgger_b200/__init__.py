@@ -31,6 +31,7 @@ from .native import (  # noqa: F401
     splitter_run,
     splitter_run_gelf,
     splitter_run_gelf_framed,
+    splitter_run_ltsv_framed,
     tz_count,
     tz_lookup,
 )

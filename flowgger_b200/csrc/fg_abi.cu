@@ -237,6 +237,8 @@ struct fg_ctx {
     const int32_t* d_static_lit_off = nullptr;
     const int32_t* d_static_kind = nullptr;
     std::vector<std::pair<std::string, std::string>> gelf_extra;
+    Buf<uint8_t> ltsv_extra;   // output.ltsv_extra as the one literal the LTSV encoder writes (fg_set_ltsv_extra)
+    int ltsv_extra_len = 0;
     fg_out_framing out_framing = FG_OUT_NONE;  // output.framing of the fused encoder (fg_set_output_framing)
     // split mode (fg_split_decode)
     Buf<uint32_t> seg;
@@ -592,8 +594,12 @@ void begin_fused(fg_ctx* c, int fmt) {
     c->gelf_now = (double)t.tv_sec + (double)t.tv_nsec / 1e9;
 }
 
-// The fused GELF encoder over the decoder's results of lines [l0, l0 + n), parse step k
-int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream_t s) {
+// The encoder a pipelined call runs after each parse step: none (the rows and side tables come back), or the GELF or
+// LTSV encoder (only the encoded records come back)
+enum Enc { ENC_NONE = 0, ENC_GELF = 1, ENC_LTSV = 2 };
+
+// The fused encoder `enc` over the decoder's results of lines [l0, l0 + n), parse step k
+int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, cudaStream_t s) {
     fg::GelfEncodeParams E{};
     E.bytes = c->bytes.d;
     E.offsets = c->offsets.d + l0;
@@ -624,11 +630,16 @@ int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream
     E.wentry_name = dev<int2>(c, T_ENTRIES, 0);
     E.wentry_val = dev<unsigned long long>(c, T_ENTRIES, 1);
     E.wentry_meta = dev<uint8_t>(c, T_ENTRIES, 2);
-    E.static_blob = c->static_blob.d;
-    E.n_static = c->n_static;
-    E.static_key_off = c->d_static_key_off;
-    E.static_lit_off = c->d_static_lit_off;
-    E.static_kind = c->d_static_kind;
+    if (enc == ENC_GELF) {
+        E.static_blob = c->static_blob.d;
+        E.n_static = c->n_static;
+        E.static_key_off = c->d_static_key_off;
+        E.static_lit_off = c->d_static_lit_off;
+        E.static_kind = c->d_static_kind;
+    } else {
+        E.static_blob = c->ltsv_extra.d;
+        E.n_static = c->ltsv_extra_len;
+    }
     E.lens = c->enc_lens.d + l0;
     E.rel = c->enc_rel.d + l0;
     E.base = c->enc_base.d + k;
@@ -644,7 +655,8 @@ int launch_encode(fg_ctx* c, int fmt, int k, int l0, int n, int tile, cudaStream
     E.out_framing = (int32_t)c->out_framing;
     // the encoder's CTAs take 256 lines (4 x the parse kernel's 64); configure_gelf_encode allowed max_tile5
     E.tile_bytes = std::min(4 * tile, c->max_tile5);
-    FG_CUDA(c, fg::launch_gelf_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
+    if (enc == ENC_GELF) FG_CUDA(c, fg::launch_gelf_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
+    else FG_CUDA(c, fg::launch_ltsv_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
     c->launches += 4;
     return FG_OK;
 }
@@ -799,12 +811,12 @@ int upload_chunk(fg_ctx* c, HostBatch& B, int k, int l0, int l1) {
 // (with `encode`, the GELF encoder after the parse), the counter snapshot, then on s_d2h once the snapshot is in: the
 // rows, or the encoder's statuses and record offsets
 int parse_step(fg_ctx* c, int fmt, int k, int l0, int n, int tile, const uint8_t* invalid, int strip, cudaStream_t s,
-               bool encode) {
+               int encode) {
     StepEvents& e = c->steps[k];
     FG_CUDA(c, cudaEventRecord(e.k0, s));
     if (int rc = launch_lines(c, fmt, l0, n, tile, invalid, strip, s)) return rc;
     if (encode)
-        if (int rc = launch_encode(c, fmt, k, l0, n, tile, s)) return rc;
+        if (int rc = launch_encode(c, encode, fmt, k, l0, n, tile, s)) return rc;
     FG_CUDA(c, cudaEventRecord(e.k1, s));
     FG_CUDA(c, cudaMemcpyAsync(c->counts.h + (size_t)k * fg::K5_COUNT, c->k.d, kCountBytes, cudaMemcpyDeviceToHost, s));
     if (encode)
@@ -830,9 +842,9 @@ struct Drain {
     bool overflow = false;
 };
 
-Drain begin_drain(fg_ctx* c, bool encode) {
+Drain begin_drain(fg_ctx* c, int encode) {
     if (encode) c->enc_base.h[0] = 0;
-    return Drain{encode};
+    return Drain{encode != ENC_NONE};
 }
 
 // Waits for the counter snapshots of the parse steps before `upto` in order and copies what each step produced back on
@@ -865,7 +877,7 @@ int end_drain(fg_ctx* c, int fmt, int steps, Drain& d, uint32_t* total, bool& ov
     return FG_OK;
 }
 
-int drain(fg_ctx* c, int fmt, int steps, bool encode, uint32_t* total, bool& overflow) {
+int drain(fg_ctx* c, int fmt, int steps, int encode, uint32_t* total, bool& overflow) {
     Drain d = begin_drain(c, encode);
     return end_drain(c, fmt, steps, d, total, overflow);
 }
@@ -1032,11 +1044,25 @@ void end_fused(fg_ctx* c, int fmt, int32_t n, float kernel_ms, float total_ms, f
     out->total_ms = total_ms;
 }
 
+// LTSVString::insert of every output.ltsv_extra pair (ltsv_encoder.rs:95-103: one leading '_' stripped from the key), each
+// with the '\t' in front that the device drops for a record's first field: `\tkey:value...`
+std::string ltsv_extra_literal(const std::vector<std::pair<std::string, std::string>>& kv) {
+    std::string lit;
+    for (const auto& [k0, v] : kv) {
+        const std::string k = !k0.empty() && k0[0] == '_' ? k0.substr(1) : k0;
+        lit.push_back('\t');
+        for (const char ch : k) lit.push_back(ch == '\n' || ch == '\t' ? ' ' : (ch == ':' ? '_' : ch));
+        lit.push_back(':');
+        for (const char ch : v) lit.push_back(ch == '\n' || ch == '\t' ? ' ' : ch);
+    }
+    return lit;
+}
+
 // The caller's lines, framed already -> H2D and the parse kernels chunk_lines lines a step, and with `encode` the GELF
 // encoder after each parse step: the pre-framed counterpart of split_stream, with the same results.  Without `encode`
 // the rows and side tables come back, with it only the encoded records.  total, kernel_ms, total_ms: as drain and finish
 // give them, zero for n == 0.
-int batch_lines(fg_ctx* c, int fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, bool encode, uint32_t* total,
+int batch_lines(fg_ctx* c, int fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, int encode, uint32_t* total,
                 float& kernel_ms, float& total_ms) {
     if (int rc = begin_call(c, (fg_format)fmt)) return rc;
     const int C = c->chunk_lines;
@@ -1070,6 +1096,19 @@ int batch_lines(fg_ctx* c, int fmt, const uint8_t* bytes, const int32_t* offsets
         if (int rc = regrow(c, fmt, total, encode ? c->enc_base.h[chunks] : 0)) return rc;
     }
     return fail(c, FG_E_CAPACITY, encode ? "output / side table overflow after regrow" : "side table overflow after regrow");
+}
+
+// decode + the encoder `enc` fused (fg_decode_encode_gelf / fg_decode_encode_ltsv)
+int decode_encode(fg_ctx* c, int enc, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
+    if (!c || !out) return FG_E_ARG;
+    begin_fused(c, (int)fmt);
+    if (int rc = check_batch(c, bytes, offsets, n)) return rc;
+    if (int rc = check_fusable(c, (int)fmt)) return rc;
+    uint32_t total[fg::K5_COUNT];
+    float kms, tms;
+    if (int rc = batch_lines(c, (int)fmt, bytes, offsets, n, enc, total, kms, tms)) return rc;
+    end_fused(c, (int)fmt, n, kms, tms, out);
+    return FG_OK;
 }
 
 // everything fg_create sets up on the device
@@ -1161,7 +1200,7 @@ int fg_decode_batch(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;
-    if (int rc = batch_lines(c, (int)fmt, bytes, offsets, n, false, total, kms, tms)) return rc;
+    if (int rc = batch_lines(c, (int)fmt, bytes, offsets, n, ENC_NONE, total, kms, tms)) return rc;
     memset(out, 0, sizeof *out);
     fill_out(c, fmt, n, total, out);
     out->kernel_ms = kms;
@@ -1261,14 +1300,31 @@ int fg_set_output_framing(fg_ctx* c, fg_out_framing framing) {
 // kernels -> D2H of the encoded records (and for LTSV the "Missing value" stops) only, chunk by chunk; the decoder's rows
 // and side tables never leave the device.
 int fg_decode_encode_gelf(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
-    if (!c || !out) return FG_E_ARG;
-    begin_fused(c, (int)fmt);
-    if (int rc = check_batch(c, bytes, offsets, n)) return rc;
-    if (int rc = check_fusable(c, (int)fmt)) return rc;
-    uint32_t total[fg::K5_COUNT];
-    float kms, tms;
-    if (int rc = batch_lines(c, (int)fmt, bytes, offsets, n, true, total, kms, tms)) return rc;
-    end_fused(c, (int)fmt, n, kms, tms, out);
+    return decode_encode(c, ENC_GELF, fmt, bytes, offsets, n, out);
+}
+
+// decode + LTSVEncoder::encode fused: the same pipeline with the LTSV encoder's kernels
+int fg_decode_encode_ltsv(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
+    return decode_encode(c, ENC_LTSV, fmt, bytes, offsets, n, out);
+}
+
+int fg_set_ltsv_extra(fg_ctx* c, int32_t n, const char* const* keys, const char* const* values) {
+    if (!c || n < 0 || (n > 0 && (!keys || !values))) return FG_E_ARG;
+    std::vector<std::pair<std::string, std::string>> kv;
+    for (int32_t k = 0; k < n; ++k) {
+        if (!keys[k] || !values[k]) return fail(c, FG_E_ARG, "output.ltsv_extra values must be strings");  // ltsv_encoder.rs:22-24
+        kv.emplace_back(keys[k], values[k]);
+    }
+    std::sort(kv.begin(), kv.end());  // a TOML table iterates its keys in byte order
+    for (size_t k = 1; k < kv.size(); ++k)
+        if (kv[k].first == kv[k - 1].first) return fail(c, FG_E_ARG, "output.ltsv_extra has a duplicate key");
+    FG_CUDA(c, cudaSetDevice(c->device));
+    FG_CUDA(c, cudaDeviceSynchronize());
+    const std::string lit = ltsv_extra_literal(kv);
+    Packer p;
+    p.add(lit);
+    if (int rc = p.upload(c, c->ltsv_extra)) return rc;
+    c->ltsv_extra_len = (int)lit.size();
     return FG_OK;
 }
 
@@ -1292,7 +1348,7 @@ namespace {
 // and with `encode` the GELF encoder after each parse step.  Without `encode` the rows and side tables come back, with
 // it only the encoded records; the line offsets come back into split_offsets.h either way.  n: records framed; total,
 // kernel_ms, total_ms: as drain and finish give them.
-int split_stream(fg_ctx* c, int fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, bool encode, int32_t& n,
+int split_stream(fg_ctx* c, int fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, int encode, int32_t& n,
                  uint32_t* total, float& kernel_ms, float& total_ms) {
     if (framing != FG_FRAME_LINE && framing != FG_FRAME_NUL) return fail(c, FG_E_ARG, "unknown framing");
     const int delim = framing == FG_FRAME_NUL ? 0 : '\n';
@@ -1402,6 +1458,21 @@ int split_stream(fg_ctx* c, int fmt, fg_framing framing, const uint8_t* stream, 
     return fail(c, FG_E_CAPACITY, encode ? "output / side table overflow after regrow" : "side table overflow after regrow");
 }
 
+// framing + decode + the encoder `enc` fused (fg_split_decode_encode_gelf / fg_split_decode_encode_ltsv)
+int split_decode_encode(fg_ctx* c, int enc, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes,
+                        fg_encoded_out* out, const int32_t** line_offsets) {
+    if (!c || !out || !line_offsets) return FG_E_ARG;
+    begin_fused(c, (int)fmt);
+    if (int rc = check_fusable(c, (int)fmt)) return rc;
+    int32_t n;
+    uint32_t total[fg::K5_COUNT];
+    float kms, tms;
+    if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, enc, n, total, kms, tms)) return rc;
+    end_fused(c, (int)fmt, n, kms, tms, out);
+    *line_offsets = c->split_offsets.h;
+    return FG_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1416,7 +1487,7 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
     int32_t n;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;
-    if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, false, n, total, kms, tms)) return rc;
+    if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, ENC_NONE, n, total, kms, tms)) return rc;
     memset(out, 0, sizeof *out);
     fill_out(c, fmt, n, total, out);
     out->line_offsets = c->split_offsets.h;
@@ -1429,16 +1500,13 @@ int fg_split_decode_framed(fg_ctx* c, fg_format fmt, fg_framing framing, const u
 // offsets and for LTSV the "Missing value" stops come back
 int fg_split_decode_encode_gelf(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
                                 const int32_t** line_offsets) {
-    if (!c || !out || !line_offsets) return FG_E_ARG;
-    begin_fused(c, (int)fmt);
-    if (int rc = check_fusable(c, (int)fmt)) return rc;
-    int32_t n;
-    uint32_t total[fg::K5_COUNT];
-    float kms, tms;
-    if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, true, n, total, kms, tms)) return rc;
-    end_fused(c, (int)fmt, n, kms, tms, out);
-    *line_offsets = c->split_offsets.h;
-    return FG_OK;
+    return split_decode_encode(c, ENC_GELF, fmt, framing, stream, nbytes, out, line_offsets);
+}
+
+// framing + decode + LTSVEncoder::encode on the device, as fg_split_decode_encode_gelf
+int fg_split_decode_encode_ltsv(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
+                                const int32_t** line_offsets) {
+    return split_decode_encode(c, ENC_LTSV, fmt, framing, stream, nbytes, out, line_offsets);
 }
 
 int fg_upload(fg_ctx* c, const uint8_t* bytes, const int32_t* offsets, int32_t n) {

@@ -353,6 +353,22 @@ FG_DEV int json_transcode_step(bytes_t p, int& i, int end, bool mode2, uint32_t&
 }
 
 
+// One step of reading a validated JSON string body p[i, end) as its unescaped bytes (the LTSV encoder writes the text,
+// not JSON): the source escape — or raw byte — at p[i] becomes 1..4 bytes in w (low byte first), i moves past it;
+// returns the byte count.  At most 4: a surrogate pair is 4 bytes of UTF-8, `\` + LF of a retry line `\` and 'n'.
+FG_DEV int json_unescape_step(bytes_t p, int& i, int end, bool mode2, uint32_t& w) {
+    KeyIter it;
+    key_iter_init(it, p, i, end, mode2);
+    w = 0;
+    int n = 0;
+    do {
+        w |= (uint32_t)key_iter_next(it) << (8 * n);
+        ++n;
+    } while (it.npend);
+    i = it.i;
+    return n;
+}
+
 // Top-level members of one line while it is being parsed: the first kMaxLocalMembers live in per-thread local
 // memory (L1-resident); an object with more members spills everything to the scratch table (rare).
 constexpr int kMaxLocalMembers = 24;

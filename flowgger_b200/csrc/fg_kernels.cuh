@@ -194,6 +194,12 @@ cudaError_t configure_gelf_encode(int max_tile_bytes);
 // fmt: the decoder whose results the encoder reads (0 = RFC5424, 1 = LTSV, 2 = GELF, 3 = RFC3164)
 cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
 size_t gelf_scan_temp_bytes(int n);
+// ---- fused LTSV encoder over the same four decoders' results (fg_ltsv_encode.cu) -------------------------------------
+// The same parameters as the GELF encoder's, except that static_blob holds output.ltsv_extra as ONE literal of n_static
+// bytes (`\tkey:value` per extra, in key order, '_' stripped and escaped on the host) and the static_key_off /
+// static_lit_off / static_kind arrays are unused.  The same scan temporary serves both.
+cudaError_t configure_ltsv_encode(int max_tile_bytes);
+cudaError_t launch_ltsv_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
 
 // RFC5424 (short lines, staged tile): 64-line CTAs — tile waits and barriers half as wide as with 128 lines
 #ifndef FG_R5_LINES  // other shapes build with -DFG_R5_LINES / -DFG_R5_MINB for A/B runs

@@ -225,28 +225,38 @@ void CudaBatchDecoder::decode_batch(const uint8_t* bytes, const int32_t* offsets
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_batch: ") + fg_last_error(ctx_));
 }
 
-void CudaBatchDecoder::set_encoder(const std::vector<std::pair<std::string, std::string>>& extra, fg_out_framing out_framing) {
+void CudaBatchDecoder::set_encoder(const CudaFusedEncoder& enc) {
     // set on every call: a host-side setting, and other callers of the same context may have changed it
-    if (fg_set_output_framing(ctx_, out_framing) != FG_OK)
+    if (fg_set_output_framing(ctx_, enc.out_framing()) != FG_OK)
         throw std::runtime_error(std::string("fg_set_output_framing: ") + fg_last_error(ctx_));
-    if (extra_valid_ && extra == extra_set_) return;
+    const std::vector<std::pair<std::string, std::string>>& extra = enc.extra();
+    const int o = enc.output() == CudaFusedEncoder::Output::Gelf ? 0 : 1;
+    if (extra_valid_[o] && extra == extra_set_[o]) return;
     std::vector<const char*> k, v;
     for (const auto& kv : extra) {
         k.push_back(kv.first.c_str());
         v.push_back(kv.second.c_str());
     }
-    if (fg_set_gelf_extra(ctx_, (int32_t)extra.size(), k.data(), v.data()) != FG_OK)
-        throw std::runtime_error(std::string("fg_set_gelf_extra: ") + fg_last_error(ctx_));
-    extra_set_ = extra;
-    extra_valid_ = true;
+    const int rc = o == 0 ? fg_set_gelf_extra(ctx_, (int32_t)extra.size(), k.data(), v.data())
+                          : fg_set_ltsv_extra(ctx_, (int32_t)extra.size(), k.data(), v.data());
+    if (rc != FG_OK) throw std::runtime_error(std::string(o == 0 ? "fg_set_gelf_extra: " : "fg_set_ltsv_extra: ") + fg_last_error(ctx_));
+    extra_set_[o] = extra;
+    extra_valid_[o] = true;
 }
 
 void CudaBatchDecoder::decode_encode_gelf(const uint8_t* bytes, const int32_t* offsets, int32_t n,
                                           const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out,
                                           fg_out_framing out_framing) {
-    set_encoder(extra, out_framing);
-    const int rc = fg_decode_encode_gelf(ctx_, fmt_, bytes, offsets, n, out);
-    if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_encode_gelf: ") + fg_last_error(ctx_));
+    decode_encode(CudaGelfEncoder(extra, out_framing), bytes, offsets, n, out);
+}
+
+void CudaBatchDecoder::decode_encode(const CudaFusedEncoder& enc, const uint8_t* bytes, const int32_t* offsets, int32_t n,
+                                     fg_encoded_out* out) {
+    set_encoder(enc);
+    const bool gelf = enc.output() == CudaFusedEncoder::Output::Gelf;
+    const int rc = (gelf ? fg_decode_encode_gelf : fg_decode_encode_ltsv)(ctx_, fmt_, bytes, offsets, n, out);
+    if (rc != FG_OK)
+        throw std::runtime_error(std::string(gelf ? "fg_decode_encode_gelf: " : "fg_decode_encode_ltsv: ") + fg_last_error(ctx_));
 }
 
 const int32_t* CudaBatchDecoder::encoded_ltsv_stops() const {
@@ -257,10 +267,17 @@ const int32_t* CudaBatchDecoder::encoded_ltsv_stops() const {
 bool CudaBatchDecoder::try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
                                                     const std::vector<std::pair<std::string, std::string>>& extra,
                                                     fg_encoded_out* out, const int32_t** line_offsets, fg_out_framing out_framing) {
-    set_encoder(extra, out_framing);
-    const int rc = fg_split_decode_encode_gelf(ctx_, fmt_, framing, stream, nbytes, out, line_offsets);
+    return try_split_decode_encode(CudaGelfEncoder(extra, out_framing), stream, nbytes, framing, out, line_offsets);
+}
+
+bool CudaBatchDecoder::try_split_decode_encode(const CudaFusedEncoder& enc, const uint8_t* stream, int64_t nbytes, fg_framing framing,
+                                               fg_encoded_out* out, const int32_t** line_offsets) {
+    set_encoder(enc);
+    const bool gelf = enc.output() == CudaFusedEncoder::Output::Gelf;
+    const int rc = (gelf ? fg_split_decode_encode_gelf : fg_split_decode_encode_ltsv)(ctx_, fmt_, framing, stream, nbytes, out, line_offsets);
     if (rc == FG_E_CAPACITY) return false;
-    if (rc != FG_OK) throw std::runtime_error(std::string("fg_split_decode_encode_gelf: ") + fg_last_error(ctx_));
+    if (rc != FG_OK)
+        throw std::runtime_error(std::string(gelf ? "fg_split_decode_encode_gelf: " : "fg_split_decode_encode_ltsv: ") + fg_last_error(ctx_));
     return true;
 }
 
@@ -514,11 +531,11 @@ bool is_invalid_utf8_status(fg_format fmt, uint32_t status) {
 
 RecordEmitter::RecordEmitter(const Encoder& encoder, std::function<void(std::vector<uint8_t>&&)> tx, std::ostream& err_out,
                              std::ostream& std_out, bool quiet_blank)
-    : encoder_(encoder), fused_(dynamic_cast<const CudaGelfEncoder*>(&encoder)), tx_(std::move(tx)), err_(err_out),
+    : encoder_(encoder), fused_(dynamic_cast<const CudaFusedEncoder*>(&encoder)), tx_(std::move(tx)), err_(err_out),
       out_(std_out), quiet_blank_(quiet_blank) {}
 
-const CudaGelfEncoder* RecordEmitter::fused_with(const CudaBatchDecoder& gpu) const {
-    return fused_ != nullptr && CudaGelfEncoder::fuses_with(gpu.format()) ? fused_ : nullptr;
+const CudaFusedEncoder* RecordEmitter::fused_with(const CudaBatchDecoder& gpu) const {
+    return fused_ != nullptr && CudaFusedEncoder::fuses_with(gpu.format()) ? fused_ : nullptr;
 }
 
 void RecordEmitter::emit(fg_format fmt, const fg_encoded_out& eo, const int32_t* stops, const uint8_t* bytes, int32_t i,
@@ -594,10 +611,10 @@ void RecordBatcher::flush_on(CudaBatchDecoder* gpu) {
     const uint8_t dummy = 0;
     const uint8_t* bytes = arena_.empty() ? &dummy : arena_.data();
     std::lock_guard<std::mutex> guard(gpu->mutex());  // held until every Record of the batch has been materialised
-    if (const CudaGelfEncoder* fused = emit_.fused_with(*gpu)) {
+    if (const CudaFusedEncoder* fused = emit_.fused_with(*gpu)) {
         // decode + encode on the device (line_splitter.rs:50-52 fused): only the encoded records come back
         fg_encoded_out eo;
-        gpu->decode_encode_gelf(bytes, offsets_.data(), n, fused->extra(), &eo, fused->out_framing());
+        gpu->decode_encode(*fused, bytes, offsets_.data(), n, &eo);
         const int32_t* stops = gpu->encoded_ltsv_stops();
         for (int32_t i = 0; i < n; ++i) {
             invalid(i);
@@ -702,11 +719,11 @@ class BlockSplitter {
     bool decode_on(CudaBatchDecoder* gpu, const uint8_t* p, int64_t n) {
         std::lock_guard<std::mutex> guard(gpu->mutex());  // held until every record of the block has been emitted
         int32_t lo, hi;
-        if (const CudaGelfEncoder* fused = emit_.fused_with(*gpu)) {
+        if (const CudaFusedEncoder* fused = emit_.fused_with(*gpu)) {
             // framing + decode + encode on the device (line_splitter.rs:17-52 fused): only the encoded records come back
             fg_encoded_out eo;
             const int32_t* lines;
-            if (!gpu->try_split_decode_encode_gelf(p, n, framing_, fused->extra(), &eo, &lines, fused->out_framing())) return false;
+            if (!gpu->try_split_decode_encode(*fused, p, n, framing_, &eo, &lines)) return false;
             const int32_t* stops = gpu->encoded_ltsv_stops();
             for (int32_t i = 0; i < eo.n; ++i) {
                 split_extent(lines, p, i, lo, hi, framing_);
@@ -1221,6 +1238,22 @@ int fgh_splitter_run_gelf_framed(void* d, const uint8_t* text, int64_t len, int3
     std::string stream, err, out;
     auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
     const CudaGelfEncoder enc(extra_of(n_extra, keys, vals), (fg_out_framing)out_framing);
+    if (run_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
+    give(stream, out_stream, out_stream_len);
+    give(err, out_stderr, out_stderr_len);
+    give(out, out_stdout, out_stdout_len);
+    return 0;
+}
+
+// fgh_splitter_run_gelf_framed with output.format = "ltsv" (CudaLtsvEncoder): the output stream exactly as the splitter
+// sent it, stderr and stdout text
+int fgh_splitter_run_ltsv_framed(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
+                                 const char* const* keys, const char* const* vals, int framing, int out_framing, uint8_t** out_stream,
+                                 int64_t* out_stream_len, uint8_t** out_stderr, int64_t* out_stderr_len, uint8_t** out_stdout,
+                                 int64_t* out_stdout_len) {
+    std::string stream, err, out;
+    auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
+    const CudaLtsvEncoder enc(extra_of(n_extra, keys, vals), (fg_out_framing)out_framing);
     if (run_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
     give(stream, out_stream, out_stream_len);
     give(err, out_stderr, out_stderr_len);

@@ -87,6 +87,8 @@ struct DeviceOptions {
 };
 
 // One GPU decoding context of a fixed format.  Single caller at a time (see mutex()).
+class CudaFusedEncoder;
+
 class CudaBatchDecoder {
    public:
     CudaBatchDecoder(fg_format fmt, const LtsvConfig& ltsv = {}, const DeviceOptions& opt = {});
@@ -124,17 +126,21 @@ class CudaBatchDecoder {
     bool try_split_decode_encode_gelf(const uint8_t* stream, int64_t nbytes, fg_framing framing,
                                       const std::vector<std::pair<std::string, std::string>>& extra, fg_encoded_out* out,
                                       const int32_t** line_offsets, fg_out_framing out_framing = FG_OUT_NONE);
-    // after one of the two fused calls on an LTSV context: where each record's "Missing value" lines stop
+    // the two calls above for either fused encoder (output format, extras and output.framing from `enc`)
+    void decode_encode(const CudaFusedEncoder& enc, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
+    bool try_split_decode_encode(const CudaFusedEncoder& enc, const uint8_t* stream, int64_t nbytes, fg_framing framing,
+                                 fg_encoded_out* out, const int32_t** line_offsets);
+    // after one of the fused calls on an LTSV context: where each record's "Missing value" lines stop
     // (fg_encoded_ltsv_stops, for ltsv_missing_values); nullptr for other formats
     const int32_t* encoded_ltsv_stops() const;
 
    private:
-    void set_encoder(const std::vector<std::pair<std::string, std::string>>& extra, fg_out_framing out_framing);
+    void set_encoder(const CudaFusedEncoder& enc);
     fg_format fmt_;
     fg_ctx* ctx_ = nullptr;
     std::mutex mu_;
-    std::vector<std::pair<std::string, std::string>> extra_set_;
-    bool extra_valid_ = false;
+    std::vector<std::pair<std::string, std::string>> extra_set_[2];  // per CudaFusedEncoder::Output
+    bool extra_valid_[2] = {false, false};
     LtsvConfig ltsv_;
     DeviceOptions opt_;
     std::string suffix_[5];
@@ -190,25 +196,50 @@ class Encoder {
 // fg_encoded_gelf_now).  `out_framing` = output.framing, applied on the device as well (fg_set_output_framing): with a
 // framing other than FG_OUT_NONE the fused paths send ONE buffer per device call, the framed records of the whole
 // batch, exactly what the Output writes, and the Output gets no merger.
-class CudaGelfEncoder : public Encoder {
+// A fused encoder, and which output format it writes: what RecordEmitter, RecordBatcher and the batching splitters need
+// to run it on the device (CudaBatchDecoder::decode_encode / try_split_decode_encode).
+class CudaFusedEncoder : public Encoder {
    public:
-    explicit CudaGelfEncoder(std::vector<std::pair<std::string, std::string>> extra = {}, fg_out_framing out_framing = FG_OUT_NONE)
-        : extra_(std::move(extra)), out_framing_(out_framing) {}
-    // the decoders whose device-resident results the fused encoder reads (fg_decode_encode_gelf)
+    enum class Output { Gelf, Ltsv };
+    // the decoders whose device-resident results the fused encoders read
     static bool fuses_with(fg_format fmt) {
         return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF;
     }
     // a lone host-side Record cannot be encoded: there is no CPU encoder behind this interface
     bool encode(Record&&, std::vector<uint8_t>&, const char** err) const override {
-        if (err) *err = "GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)";
+        if (err)
+            *err = output_ == Output::Gelf ? "GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)"
+                                           : "LTSVEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)";
         return false;
     }
+    Output output() const { return output_; }
+    // output.gelf_extra or output.ltsv_extra
     const std::vector<std::pair<std::string, std::string>>& extra() const { return extra_; }
     fg_out_framing out_framing() const { return out_framing_; }
 
+   protected:
+    CudaFusedEncoder(Output output, std::vector<std::pair<std::string, std::string>> extra, fg_out_framing out_framing)
+        : output_(output), extra_(std::move(extra)), out_framing_(out_framing) {}
+
    private:
+    Output output_;
     std::vector<std::pair<std::string, std::string>> extra_;
     fg_out_framing out_framing_;
+};
+
+class CudaGelfEncoder : public CudaFusedEncoder {
+   public:
+    explicit CudaGelfEncoder(std::vector<std::pair<std::string, std::string>> extra = {}, fg_out_framing out_framing = FG_OUT_NONE)
+        : CudaFusedEncoder(Output::Gelf, std::move(extra), out_framing) {}
+};
+
+// encoder/ltsv_encoder.rs:10-30: output.format = "ltsv", fused with the decoder on the GPU as CudaGelfEncoder is
+// (fg_decode_encode_ltsv).  `extra` = output.ltsv_extra (written in byte order of its keys), `out_framing` =
+// output.framing (the caller resolves the reference's "line" default for ltsv, mod.rs:444-460).
+class CudaLtsvEncoder : public CudaFusedEncoder {
+   public:
+    explicit CudaLtsvEncoder(std::vector<std::pair<std::string, std::string>> extra = {}, fg_out_framing out_framing = FG_OUT_NONE)
+        : CudaFusedEncoder(Output::Ltsv, std::move(extra), out_framing) {}
 };
 
 // What RecordBatcher and the batching splitters do with each record of a batch decoded on the device, one record at a
@@ -219,8 +250,8 @@ class RecordEmitter {
    public:
     RecordEmitter(const Encoder& encoder, std::function<void(std::vector<uint8_t>&&)> tx, std::ostream& err_out,
                   std::ostream& std_out, bool quiet_blank);
-    // the encoder when it runs fused with the decoder of `gpu` (CudaGelfEncoder::fuses_with), else nullptr
-    const CudaGelfEncoder* fused_with(const CudaBatchDecoder& gpu) const;
+    // the encoder when it runs fused with the decoder of `gpu` (CudaFusedEncoder::fuses_with), else nullptr
+    const CudaFusedEncoder* fused_with(const CudaBatchDecoder& gpu) const;
     // record i of a fused call on a decoder of format `fmt`; `stops` = CudaBatchDecoder::encoded_ltsv_stops()
     void emit(fg_format fmt, const fg_encoded_out& eo, const int32_t* stops, const uint8_t* bytes, int32_t i, int32_t lo,
               int32_t hi);
@@ -234,7 +265,7 @@ class RecordEmitter {
    private:
     void reject(fg_format fmt, uint32_t status, const char* err, const uint8_t* bytes, int32_t lo, int32_t hi);
     const Encoder& encoder_;
-    const CudaGelfEncoder* fused_;
+    const CudaFusedEncoder* fused_;
     std::function<void(std::vector<uint8_t>&&)> tx_;
     std::ostream& err_;
     std::ostream& out_;

@@ -107,6 +107,9 @@ def load_cuda() -> C.CDLL:
         L.fg_decode_encode_gelf.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(FgEncodedOut)]
         L.fg_split_decode_encode_gelf.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.POINTER(FgEncodedOut),
                                                   C.POINTER(C.POINTER(C.c_int32))]
+        L.fg_set_ltsv_extra.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p)]
+        L.fg_decode_encode_ltsv.argtypes = L.fg_decode_encode_gelf.argtypes
+        L.fg_split_decode_encode_ltsv.argtypes = L.fg_split_decode_encode_gelf.argtypes
         L.fg_encoded_ltsv_stops.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
         L.fg_encoded_gelf_now.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         L.fg_set_output_framing.argtypes = [C.c_void_p, C.c_int]
@@ -148,6 +151,7 @@ def load_host() -> C.CDLL:
                                             C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]
         L.fgh_splitter_run_gelf_framed.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int64, C.c_int, C.POINTER(C.c_char_p),
                                                    C.POINTER(C.c_char_p), C.c_int, C.c_int] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
+        L.fgh_splitter_run_ltsv_framed.argtypes = L.fgh_splitter_run_gelf_framed.argtypes
         L.fgh_splitter_run.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int64, C.c_int32, C.c_int64] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         _host = L
     return _host
@@ -415,11 +419,30 @@ class BatchDecoder:
         with "_"), strings re-escaped from their unescaped text, and gelf_now() as "timestamp" when the object has none.
         With copy=False the arrays are views of the context's pinned buffers (valid until the
         next call)."""
+        return self._decode_encode("fg_decode_encode_gelf", data, offsets, copy)
+
+    def set_ltsv_extra(self, extra: dict[str, str]) -> None:
+        """output.ltsv_extra of LTSVEncoder::new (ltsv_encoder.rs:10-30); written in byte order of the keys."""
+        self._check(self.L.fg_set_ltsv_extra(self.ctx, *_extra_arrays(extra)), "fg_set_ltsv_extra")
+
+    def decode_encode_ltsv(self, data: np.ndarray, offsets: np.ndarray, copy: bool = True):
+        """decode + LTSVEncoder::encode fused on the device (fg_decode_encode_ltsv), for the same four decoders as
+        decode_encode_gelf and with the same results: (LTSV bytes, int64 offsets[n+1], status uint8[n], kernel ms).  A
+        record is `key:value` fields separated by tabs in Record order: the SD pairs (names without their leading "_"),
+        the extras, host, time (Rust's Display for f64), then message, full_message, level, facility, appname, procid and
+        msgid where the Record has them."""
+        return self._decode_encode("fg_decode_encode_ltsv", data, offsets, copy)
+
+    def split_decode_encode_ltsv(self, stream: np.ndarray, framing: int = 0, copy: bool = True):
+        """split_decode_encode_gelf with the LTSV encoder (fg_split_decode_encode_ltsv)."""
+        return self._split_decode_encode("fg_split_decode_encode_ltsv", stream, framing, copy)
+
+    def _decode_encode(self, fn: str, data: np.ndarray, offsets: np.ndarray, copy: bool):
         assert data.dtype == np.uint8 and offsets.dtype == np.int32
         out = FgEncodedOut()
         n = len(offsets) - 1
         self._keep = (data, offsets)
-        self._check(self.L.fg_decode_encode_gelf(self.ctx, self.fmt, _ptr(data), _ptr(offsets), n, C.byref(out)), "fg_decode_encode_gelf")
+        self._check(getattr(self.L, fn)(self.ctx, self.fmt, _ptr(data), _ptr(offsets), n, C.byref(out)), fn)
         self._last_encoded_n = n
         buf, offs, status = _encoded_views(out)
         if copy:
@@ -432,12 +455,14 @@ class BatchDecoder:
         int32[n+1] in `stream` with their terminators, kernel ms).  A record that is not UTF-8 has status 76
         ("Invalid UTF-8 input") and an empty JSON record.
         With copy=False the arrays are views of the context's pinned buffers (valid until the next call)."""
+        return self._split_decode_encode("fg_split_decode_encode_gelf", stream, framing, copy)
+
+    def _split_decode_encode(self, fn: str, stream: np.ndarray, framing: int, copy: bool):
         assert stream.dtype == np.uint8
         out = FgEncodedOut()
         lo = C.POINTER(C.c_int32)()
         self._keep = (stream,)
-        self._check(self.L.fg_split_decode_encode_gelf(self.ctx, self.fmt, framing, _ptr(stream), len(stream), C.byref(out), C.byref(lo)),
-                    "fg_split_decode_encode_gelf")
+        self._check(getattr(self.L, fn)(self.ctx, self.fmt, framing, _ptr(stream), len(stream), C.byref(out), C.byref(lo)), fn)
         n = out.n
         self._last_encoded_n = n
         buf, offs, status = _encoded_views(out)
@@ -615,6 +640,16 @@ def splitter_run_gelf_framed(dec: "BatchDecoder", text: bytes, out_framing: int,
     H = load_host()
     n_extra, keys, vals = _extra_arrays(extra)
     return _run_splitter(lambda o: H.fgh_splitter_run_gelf_framed(dec._h, text, len(text), max_lines, max_bytes, n_extra, keys,
+                                                                  vals, framing, out_framing, *o))
+
+
+def splitter_run_ltsv_framed(dec: "BatchDecoder", text: bytes, out_framing: int, extra: dict[str, str] | None = None,
+                             max_lines: int = 1 << 16, max_bytes: int = 16 << 20, framing: int = 0) -> tuple[bytes, bytes, bytes]:
+    """splitter_run_gelf_framed with output.format = "ltsv" (CudaLtsvEncoder, output.ltsv_extra = extra): returns (the
+    output stream exactly as the splitter sent it, stderr text, stdout text)."""
+    H = load_host()
+    n_extra, keys, vals = _extra_arrays(extra)
+    return _run_splitter(lambda o: H.fgh_splitter_run_ltsv_framed(dec._h, text, len(text), max_lines, max_bytes, n_extra, keys,
                                                                   vals, framing, out_framing, *o))
 
 

@@ -308,6 +308,27 @@ int fg_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_
  * nbytes > max_batch_bytes or more records than max_batch_lines -> FG_E_CAPACITY (the context stays usable). */
 int fg_split_decode_encode_gelf(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */, fg_framing framing,
                                 const uint8_t* stream, int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
+/* output.format = "ltsv" (encoder/ltsv_encoder.rs:10-123), the same four input formats:
+ *     LTSVEncoder::new(&Config)   ltsv_encoder.rs:10-30   -> fg_set_ltsv_extra (output.ltsv_extra)
+ *     Encoder::encode(Record)     ltsv_encoder.rs:66-123  -> fg_decode_encode_ltsv / fg_split_decode_encode_ltsv
+ * Record i is the text LTSVEncoder::encode returns: `key:value` fields separated by '\t', in Record order with no sorting
+ * and no de-duplication — every SD pair (its name without one leading '_': for LTSV input name + type suffix, for GELF
+ * input the member's name without its '_'), the extras, host (as it is, "" included), time (Record.ts as Rust's
+ * Display for f64: shortest round-trip digits, positional, no exponent: 1, 1000000000000000000000, 0.0000001, NaN, inf,
+ * -0), then message, full_message, level, facility, appname, procid, msgid each only when the Record has it (RFC5424:
+ * all; RFC3164: no appname / procid / msgid, level and facility only with a <PRI>; LTSV and GELF: no facility, appname,
+ * procid or msgid).  In keys '\n' and '\t' become ' ' and ':' becomes '_'; in values '\t' and '\n' become ' '; nothing
+ * else is escaped.  Typed values: true / false, f64 as above, decimal integers, null as "".  Everything else —
+ * fg_encoded_out, statuses, empty rejected records, output.framing (fg_set_output_framing: the caller resolves the
+ * reference's "line" default for ltsv), fg_encoded_ltsv_stops, fg_encoded_gelf_now, FG_E_CAPACITY, the input format
+ * rule — is exactly as for the GELF twins above.
+ * fg_set_ltsv_extra: the extras are written in byte order of their keys (a TOML table); a duplicate key or a NULL string
+ * -> FG_E_ARG with the extras unchanged; n = 0 clears them. */
+int fg_set_ltsv_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
+int fg_decode_encode_ltsv(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */,
+                          const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
+int fg_split_decode_encode_ltsv(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */, fg_framing framing,
+                                const uint8_t* stream, int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
 /* The one side effect of LTSVDecoder::decode, println!("Missing value for name '{}'") for every tab-separated part
  * without ':' that the decode loop reached (ltsv_decoder.rs:99), for the records of the last fused call on an LTSV
  * context.  *stop ([out->n], valid until the next call on the context): -1 when record i printed nothing; else the offset,

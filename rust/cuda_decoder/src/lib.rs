@@ -46,7 +46,7 @@ struct Ctx {
     suffix: [Option<String>; 5],
     spec: CtxSpec,
     max_bytes: usize,                        // max_batch_bytes as fg_create took it
-    extra: Option<Vec<(String, String)>>,    // the output.gelf_extra last set on the context
+    extra: [Option<Vec<(String, String)>>; 2],  // the output.gelf_extra / output.ltsv_extra last set on the context
 }
 unsafe impl Send for Ctx {}
 impl Drop for Ctx {
@@ -139,7 +139,7 @@ impl CudaDecoder {
         }
         let max_bytes = if max_bytes > 0 { (max_bytes as usize).min(0x7FFF_FFC0) } else { 256 << 20 };  // fg_create's default and cap
         let suffix = spec.suffix.clone();
-        CudaDecoder { ctx: Arc::new(Mutex::new(Ctx { raw, fmt, suffix, spec, max_bytes, extra: None })) }
+        CudaDecoder { ctx: Arc::new(Mutex::new(Ctx { raw, fmt, suffix, spec, max_bytes, extra: [None, None] })) }
     }
 
     /// max_batch_bytes of the context
@@ -223,29 +223,37 @@ impl CudaDecoder {
     /// `out_framing` (output.framing, `fg_set_output_framing`).  Then `all(bytes)` with the framed records of the whole
     /// call, the bytes one Output writes for them.  false (nothing decoded) when the stream does not fit the context.
     pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String]), G: FnOnce(&[u8])>(
-        &self, stream: &[u8], extra: &[(String, String)], out_framing: fg_out_framing, mut f: F, all: G) -> bool {
+        &self, stream: &[u8], extra: &[(String, String)], out_framing: fg_out_framing, f: F, all: G) -> bool {
+        self.split_decode_encode(FusedOutput::Gelf, stream, extra, out_framing, f, all)
+    }
+
+    /// `split_decode_encode_gelf` for either fused encoder: `output` = output.format, `extra` = its extras
+    /// (output.gelf_extra or output.ltsv_extra); with `FusedOutput::Ltsv` the records are `LTSVEncoder::encode`'s text
+    /// (`fg_split_decode_encode_ltsv`).
+    pub fn split_decode_encode<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String]), G: FnOnce(&[u8])>(
+        &self, output: FusedOutput, stream: &[u8], extra: &[(String, String)], out_framing: fg_out_framing, mut f: F, all: G) -> bool {
         let mut ctx = self.ctx.lock().unwrap();
         assert_eq!(unsafe { fg_set_output_framing(ctx.raw, out_framing) }, 0);
-        if ctx.extra.as_deref() != Some(extra) {
+        let o = output as usize;
+        if ctx.extra[o].as_deref() != Some(extra) {
             let keys: Vec<CString> = extra.iter().map(|(k, _)| CString::new(k.as_str()).unwrap()).collect();
             let vals: Vec<CString> = extra.iter().map(|(_, v)| CString::new(v.as_str()).unwrap()).collect();
             let kp: Vec<*const c_char> = keys.iter().map(|s| s.as_ptr()).collect();
             let vp: Vec<*const c_char> = vals.iter().map(|s| s.as_ptr()).collect();
-            assert_eq!(unsafe { fg_set_gelf_extra(ctx.raw, kp.len() as i32, kp.as_ptr(), vp.as_ptr()) }, 0);
-            ctx.extra = Some(extra.to_vec());
+            let set = match output { FusedOutput::Gelf => fg_set_gelf_extra, FusedOutput::Ltsv => fg_set_ltsv_extra };
+            assert_eq!(unsafe { set(ctx.raw, kp.len() as i32, kp.as_ptr(), vp.as_ptr()) }, 0);
+            ctx.extra[o] = Some(extra.to_vec());
         }
         let mut out: fg_encoded_out = unsafe { std::mem::zeroed() };
         let mut lines: *const i32 = ptr::null();
-        let rc = unsafe {
-            fg_split_decode_encode_gelf(ctx.raw, ctx.fmt, fg_framing_FG_FRAME_LINE, stream.as_ptr(), stream.len() as i64, &mut out,
-                                        &mut lines)
-        };
+        let call = match output { FusedOutput::Gelf => fg_split_decode_encode_gelf, FusedOutput::Ltsv => fg_split_decode_encode_ltsv };
+        let rc = unsafe { call(ctx.raw, ctx.fmt, fg_framing_FG_FRAME_LINE, stream.as_ptr(), stream.len() as i64, &mut out, &mut lines) };
         if rc == FG_E_CAPACITY {
             return false;
         }
         if rc != 0 {
             let e = unsafe { CStr::from_ptr(fg_last_error(ctx.raw)) }.to_string_lossy().into_owned();
-            panic!("fg_split_decode_encode_gelf: {}", e);
+            panic!("fused decode + encode: {}", e);
         }
         let n = out.n as usize;
         let offs = unsafe { std::slice::from_raw_parts(lines, n + 1) };
@@ -589,6 +597,19 @@ pub fn fuses_with_gelf(input_format: &str) -> bool {
     matches!(input_format, "rfc5424" | "rfc3164" | "ltsv" | "gelf")
 }
 
+/// The `input.format` values whose decoder runs fused with the LTSV encoder on the device (`fg_decode_encode_ltsv`,
+/// `fg_split_decode_encode_ltsv`): the same four; `FusedLtsvLineSplitter` takes a `CudaDecoder` of one of them.
+pub fn fuses_with_ltsv(input_format: &str) -> bool {
+    fuses_with_gelf(input_format)
+}
+
+/// The output format of a fused encoder (output.format = "gelf" or "ltsv")
+#[derive(Clone, Copy, PartialEq, Eq, Debug)]
+pub enum FusedOutput {
+    Gelf = 0,
+    Ltsv = 1,
+}
+
 /// The device framing of an `output.framing` value, as `mod.rs:453-460` picks the merger (panics on an unknown one, as
 /// the reference does)
 pub fn out_framing_of(output_framing: &str) -> fg_out_framing {
@@ -619,19 +640,40 @@ pub struct FusedGelfLineSplitter {
 
 impl<T: Read> Splitter<T> for FusedGelfLineSplitter {
     fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
-        let max_bytes = self.max_bytes.min(self.gpu.capacity_bytes());
-        let framed = self.out_framing != fg_out_framing_FG_OUT_NONE;
-        run_blocks(buf_reader, max_bytes, |block| {
-            decode_fitting(&self.gpu, block, &mut |gpu: &CudaDecoder, part: &[u8]| {
-                gpu.split_decode_encode_gelf(part, &self.extra, self.out_framing, |line, r, side| {
-                    for s in side { println!("{}", s); }  // ltsv_decoder.rs:99
-                    match r {
-                        Ok(json) => if !framed { tx.send(json.to_vec()).unwrap() },
-                        Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
-                        Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
-                    }
-                }, |all| if framed && !all.is_empty() { tx.send(all.to_vec()).unwrap() })
-            })
-        });
+        run_fused(&self.gpu, FusedOutput::Gelf, &self.extra, self.out_framing, self.max_bytes, buf_reader, tx)
     }
+}
+
+/// `output.format = "ltsv"` with `input.format` one of `fuses_with_ltsv`: `FusedGelfLineSplitter` with the LTSV encoder
+/// (`fg_split_decode_encode_ltsv`, replaces Decoder::decode + LTSVEncoder::encode, ltsv_encoder.rs:66-123).  The caller
+/// resolves output.framing's default, "line" for ltsv (mod.rs:444-460).
+pub struct FusedLtsvLineSplitter {
+    pub gpu: CudaDecoder,
+    pub extra: Vec<(String, String)>,   // output.ltsv_extra (ltsv_encoder.rs:10-30), in byte order of the keys
+    pub out_framing: fg_out_framing,    // output.framing (mod.rs:444-460), resolved by the caller
+    pub max_bytes: usize,
+}
+
+impl<T: Read> Splitter<T> for FusedLtsvLineSplitter {
+    fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
+        run_fused(&self.gpu, FusedOutput::Ltsv, &self.extra, self.out_framing, self.max_bytes, buf_reader, tx)
+    }
+}
+
+fn run_fused<T: Read>(gpu: &CudaDecoder, output: FusedOutput, extra: &[(String, String)], out_framing: fg_out_framing, max_bytes: usize,
+                      buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>) {
+    let max_bytes = max_bytes.min(gpu.capacity_bytes());
+    let framed = out_framing != fg_out_framing_FG_OUT_NONE;
+    run_blocks(buf_reader, max_bytes, |block| {
+        decode_fitting(gpu, block, &mut |gpu: &CudaDecoder, part: &[u8]| {
+            gpu.split_decode_encode(output, part, extra, out_framing, |line, r, side| {
+                for s in side { println!("{}", s); }  // ltsv_decoder.rs:99
+                match r {
+                    Ok(rec) => if !framed { tx.send(rec.to_vec()).unwrap() },
+                    Err("Invalid UTF-8 input") => { let _ = writeln!(stderr(), "Invalid UTF-8 input"); }   // line_splitter.rs:22-25
+                    Err(e) => { let _ = writeln!(stderr(), "{}: [{}]", e, String::from_utf8_lossy(line).trim()); }  // :37-39
+                }
+            }, |all| if framed && !all.is_empty() { tx.send(all.to_vec()).unwrap() })
+        })
+    });
 }
