@@ -618,6 +618,9 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
     if (fmt == FG_FMT_GELF) {
         E.gelf_now = c->gelf_now;
         E.gelf_entries = c->k.d + fg::K5_ENTRIES;
+        // a line longer than the LTSV encoder's segment length field (2^29 - 1 bytes, the GELF encoder's is 2^30 - 1) may
+        // hold a string with escapes that no segment holds: long_json_span_kernel looks for one
+        if (c->max_bytes >= ((size_t)1 << 29)) E.long_json_span = c->k.d + fg::K5_LONG_JSON_SPAN;
     }
     if (fmt == FG_FMT_LTSV) {
         E.ltsv_suffix = c->ltsv.suffix;
@@ -657,7 +660,7 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
     E.tile_bytes = std::min(4 * tile, c->max_tile5);
     if (enc == ENC_GELF) FG_CUDA(c, fg::launch_gelf_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
     else FG_CUDA(c, fg::launch_ltsv_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
-    c->launches += 4;
+    c->launches += E.long_json_span ? 5 : 4;
     return FG_OK;
 }
 
@@ -888,6 +891,8 @@ int finish(fg_ctx* c, int steps, const uint32_t* total, std::chrono::steady_cloc
            float& total_ms) {
     FG_CUDA(c, cudaStreamSynchronize(c->s_d2h));
     if (total[fg::K5_BAD_OFFSETS]) return fail(c, FG_E_ARG, "offsets must be non-decreasing and within max_batch_bytes");
+    if (total[fg::K5_LONG_JSON_SPAN])
+        return fail(c, FG_E_CAPACITY, "a GELF string with escapes is too long to encode (GELF output: 1 GiB or more, LTSV output: 512 MiB or more)");
     kernel_ms = 0.f;
     for (int k = 0; k < steps; ++k) {
         float ms = 0.f;

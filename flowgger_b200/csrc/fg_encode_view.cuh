@@ -327,13 +327,43 @@ __device__ __forceinline__ bool load_pair_gelf(const GelfEncodeParams& P, const 
     return true;
 }
 
+// Whether a GELF row holds a span with JSON escapes longer than `limit` bytes, the longest span an encoder's segment
+// length field holds.  Such a span is not cut into segments (a cut could split an escape): long_json_span_kernel flags
+// it and the call fails.  A member name is measured with the '_' load_pair_gelf strips (one byte, or the six of
+// \u005f): a name up to six bytes shorter than the limit is refused too, which errs on the safe side.
+__device__ __forceinline__ bool json_span_over(const GelfEncodeParams& P, const RecView& r, int limit) {
+    if (((r.flags & kHostEsc) && r.host.len > limit) || ((r.flags & kMsgEsc) && r.msg.len > limit) ||
+        ((r.flags & kFullEsc) && r.full.len > limit))
+        return true;
+    for (uint32_t e = r.first; e < r.first + r.count; ++e) {
+        const uint32_t m = P.wentry_meta[e];
+        if ((m & kEmNameEsc) && P.wentry_name[e].y > limit) return true;
+        if ((m & 0x07u) == 0u && (m & kEmUnescape) && (int)(P.wentry_val[e] >> 32) > limit) return true;
+    }
+    return false;
+}
+
+// GELF source: sets *P.long_json_span when a line holds a span json_span_over finds.  Only a line longer than `limit`
+// can hold one, so the launchers run this kernel, one thread per line, only for a context whose lines may be that long
+// (fg_abi.cu sets P.long_json_span then), and the size and write kernels carry no code for it.
+__global__ void long_json_span_kernel(const __grid_constant__ GelfEncodeParams P, int limit) {
+    const int i = blockIdx.x * blockDim.x + (int)threadIdx.x;
+    if (*P.bad_offsets || i >= P.n || P.offsets[i + 1] - P.offsets[i] <= limit) return;
+    RecView r;
+    load_view_gelf(P, ByteSource{P.bytes, 0}, i, r);
+    if (r.ok && json_span_over(P, r, limit)) *P.long_json_span = 1u;
+}
+
 // The record sources the kernels are instantiated for.  kSd: the record may carry structured data.  kOptional:
 // application_name and process_id are None, and level is None without a severity.  kLtsv: pairs are LtsvKey / LtsvVal
 // (composed keys, typed values), and the size pass writes the "Missing value" stop of every line.  kGelf: pairs are
 // GelfKey / GelfVal, full_message may be None, and spans may hold JSON escapes.  kWriteCtas: the CTAs per SM
 // gelf_write_kernel is allocated for (launch bounds; 0: ptxas's choice).  It holds each write kernel at the registers it
 // had before the output.framing code was added to it (From3164 48, FromGelf 64): without the bound, ptxas cut FromGelf to
-// 48 registers with 214 B of spill stores, 3-4 % slower on the GELF workload.
+// 48 registers with 214 B of spill stores, 3-4 % slower on the GELF workload.  The LTSV encoder's kernels
+// (fg_ltsv_encode.cu) have no such bound; ptxas (CUDA 12.9, sm_90a) gives its size kernels 64 / 48 / 48 / 48 registers
+// and its write kernels 64 / 62 / 64 / 48 (From5424 / From3164 / FromLtsv / FromGelf), with spill stores only for
+// FromGelf (50 B size, 52 B write).
 struct From5424 {
     static constexpr bool kSd = true, kOptional = false, kLtsv = false, kGelf = false;
     static constexpr int kWriteCtas = 0;

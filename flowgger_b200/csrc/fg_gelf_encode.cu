@@ -153,6 +153,7 @@ struct Seg {
 constexpr int kMaxSegs = 56;  // a record with more segments is emitted in several windows (rebuilt with `skip`)
 constexpr int kEscBit = (int)0x80000000u;
 constexpr int kJsonBit = 0x40000000;
+constexpr int kMaxSegLen = kJsonBit - 1;  // the longest span one segment holds
 __device__ const uint8_t kLit[] = "{}\",\"_\":\"\"unknown\"\"-\"\"1.1\"01234567";
 //                                 0 1 2 3..5 6..8 9..17      18..20 21..25 26..33
 enum { L_OPEN = 0, L_CLOSE = 1, L_QUOTE = 2, L_PAIR = 3 /* ,"_ */, L_MID = 6 /* ":" */, L_UNKNOWN = 9, L_DASH = 18, L_V11 = 21, L_DIGITS = 26 };
@@ -181,9 +182,13 @@ struct SegList {
     // a number whose text does not exist yet (LTSV): the segment points at its 8 value bytes in the side table and holds
     // its fg_ltsv_type as length; run_segments formats it when it reaches the segment
     __device__ __forceinline__ void num(const unsigned long long* at, uint32_t tag) { push((const uint8_t*)at, (int)tag, false); }
-    // GELF: a string span as serde_json writes its unescaped text; json = the span holds JSON escapes
+    // GELF: a string span as serde_json writes its unescaped text; json = the span holds JSON escapes.  A span longer than
+    // kMaxSegLen is cut into several segments, which is exact because the escapes of a copied span are per byte (the
+    // other sources need no cut: their byte loop reads bit 30 as length).  A span with JSON escapes is not cut (a cut
+    // could split an escape): long_json_span_kernel fails the call for one that long.
     __device__ __forceinline__ void text(const uint8_t* p, int len, bool json) {
         if (!json) {
+            for (; len > kMaxSegLen; p += kMaxSegLen, len -= kMaxSegLen) push(p, kMaxSegLen, true);
             push(p, len, true);
         } else if (len > 0) {
             push(p, len | kJsonBit, true);
@@ -688,7 +693,9 @@ cudaError_t launch_gelf_encode(int fmt, const GelfEncodeParams& p, void* d_scan_
     switch (fmt) {
         case 0: return launch_src<From5424>(p, d_scan_temp, scan_temp_bytes, stream);
         case 1: return launch_src<FromLtsv>(p, d_scan_temp, scan_temp_bytes, stream);
-        case 2: return launch_src<FromGelf>(p, d_scan_temp, scan_temp_bytes, stream);
+        case 2:
+            if (p.long_json_span) long_json_span_kernel<<<(p.n + kEncLines - 1) / kEncLines, kEncLines, 0, stream>>>(p, kMaxSegLen);
+            return launch_src<FromGelf>(p, d_scan_temp, scan_temp_bytes, stream);
         case 3: return launch_src<From3164>(p, d_scan_temp, scan_temp_bytes, stream);
         default: return cudaErrorInvalidValue;
     }

@@ -105,7 +105,7 @@ static_assert(sizeof(WideRow) == 72, "WideRow must be 72 bytes");
 
 // the counter block of a context: K5_BAD_OFFSETS is set by check_offsets_kernel; K5_COUNT words are snapshotted per chunk
 enum { K5_ENTRIES = 0, K5_ARENA = 1, K5_WIDE_ROWS = 2, K5_WIDE_ENTRIES = 3, K5_ESC_LIST = 4, K5_WIDE_LIST = 5, K5_BAD_OFFSETS = 6,
-       K5_COUNT = 8 };
+       K5_LONG_JSON_SPAN = 7, K5_COUNT = 8 };
 
 struct Parse5424Params {
     const uint8_t* bytes;
@@ -187,6 +187,10 @@ struct GelfEncodeParams {
     // rows the GELF parse kernels placed in the side table so far: past wentry_cap, a row's {first, count} may name
     // rows of other lines (the batch is redone after the regrow), so no row is read
     const uint32_t* gelf_entries;
+    // GELF source, a context whose lines may pass 2^29 bytes: set by long_json_span_kernel when a span with JSON escapes
+    // is longer than the encoder's segment length field holds (the call fails with FG_E_CAPACITY: such a span is not cut
+    // into segments); nullptr: the kernel is not launched
+    uint32_t* long_json_span;
     // output.framing (fg_out_frame.cuh: OutFraming) applied to every record written
     int32_t out_framing;
 };

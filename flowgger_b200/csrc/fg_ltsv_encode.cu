@@ -53,6 +53,16 @@ struct LtsvSegs {
         }
         ++idx;
     }
+    // a span of text: one longer than the length field is cut into several segments, which is exact because the
+    // replacements are per byte.  A span with JSON escapes is not cut (a cut could split an escape): the size kernel
+    // fails the call for one that long (long_json_span_kernel), and its record stays inside the span.
+    __device__ __forceinline__ void span(const uint8_t* q, int l, uint32_t kind) {
+        if (kind < SK_JSON_VAL)
+            for (; l > kLenMask; q += kLenMask, l -= kLenMask) push(q, kLenMask, kind);
+        else
+            l &= kLenMask;
+        push(q, l, kind);
+    }
     __device__ __forceinline__ void lit(int at, int l) { push(kLtsvLit + at, l, SK_RAW); }
     // `\tname:` of a fixed field, the tab dropped for the record's first field
     __device__ __forceinline__ void field(int at, int l) {
@@ -66,7 +76,7 @@ struct LtsvSegs {
     __device__ __forceinline__ void num(unsigned long long v, uint32_t tag) {
         push(reinterpret_cast<const uint8_t*>(v), (int)tag, SK_NUM);
     }
-    __device__ __forceinline__ void text(Span s, bool json) { push(s.p, s.len, json ? SK_JSON_VAL : SK_VAL); }
+    __device__ __forceinline__ void text(Span s, bool json) { span(s.p, s.len, json ? SK_JSON_VAL : SK_VAL); }
 };
 
 // one SD pair of the record
@@ -77,20 +87,20 @@ __device__ __forceinline__ void ltsv_pair(const GelfEncodeParams& P, const ByteS
     if (!Src::pair(P, B, r, e, k, v)) return;  // an RFC5424 element header
     L.key_start();
     if constexpr (Src::kLtsv) {  // '_' + name + suffix: the name and the type's suffix
-        L.push(k.name.p, k.name.len, SK_KEY);
+        L.span(k.name.p, k.name.len, SK_KEY);
         L.push(k.suffix.p, k.suffix.len, SK_KEY);
         L.lit(LT_COLON, 1);
-        if (v.tag == 0u) L.push(B.at((int)(uint32_t)v.v), (int)(v.v >> 32), SK_VAL);
+        if (v.tag == 0u) L.span(B.at((int)(uint32_t)v.v), (int)(v.v >> 32), SK_VAL);
         else L.num(v.v, v.tag);
     } else if constexpr (Src::kGelf) {  // the name without its '_' (load_pair_gelf), strings as their unescaped text
-        L.push(k.name.p, k.name.len, k.esc ? SK_JSON_KEY : SK_KEY);
+        L.span(k.name.p, k.name.len, k.esc ? SK_JSON_KEY : SK_KEY);
         L.lit(LT_COLON, 1);
-        if (v.tag == 0u) L.push(B.at((int)(uint32_t)v.v), (int)(v.v >> 32), v.esc ? SK_JSON_VAL : SK_VAL);
+        if (v.tag == 0u) L.span(B.at((int)(uint32_t)v.v), (int)(v.v >> 32), v.esc ? SK_JSON_VAL : SK_VAL);
         else if (v.tag != 5u) L.num(v.v, v.tag);  // Null: ""
     } else {  // RFC5424: the name as written (the decoder's '_' is the one stripped)
-        L.push(k.p, k.len, SK_KEY);
+        L.span(k.p, k.len, SK_KEY);
         L.lit(LT_COLON, 1);
-        L.push(v.p, v.len, SK_VAL);
+        L.span(v.p, v.len, SK_VAL);
     }
 }
 
@@ -99,7 +109,7 @@ __device__ __forceinline__ void build_ltsv(const GelfEncodeParams& P, const Byte
     if constexpr (Src::kSd)
         for (uint32_t e = r.first; e < r.first + r.count; ++e) ltsv_pair<Src>(P, B, r, e, L);
     if (P.n_static > 0) {  // output.ltsv_extra: `\tkey:value` per extra
-        L.push(P.static_blob + (L.first ? 1 : 0), P.n_static - (L.first ? 1 : 0), SK_RAW);
+        L.span(P.static_blob + (L.first ? 1 : 0), P.n_static - (L.first ? 1 : 0), SK_RAW);
         L.first = false;
     }
     const bool g = Src::kGelf;
@@ -300,7 +310,9 @@ cudaError_t launch_ltsv_encode(int fmt, const GelfEncodeParams& p, void* d_scan_
     switch (fmt) {
         case 0: return launch_ltsv_src<From5424>(p, d_scan_temp, scan_temp_bytes, stream);
         case 1: return launch_ltsv_src<FromLtsv>(p, d_scan_temp, scan_temp_bytes, stream);
-        case 2: return launch_ltsv_src<FromGelf>(p, d_scan_temp, scan_temp_bytes, stream);
+        case 2:
+            if (p.long_json_span) long_json_span_kernel<<<(p.n + kEncLines - 1) / kEncLines, kEncLines, 0, stream>>>(p, kLenMask);
+            return launch_ltsv_src<FromGelf>(p, d_scan_temp, scan_temp_bytes, stream);
         case 3: return launch_ltsv_src<From3164>(p, d_scan_temp, scan_temp_bytes, stream);
         default: return cudaErrorInvalidValue;
     }
