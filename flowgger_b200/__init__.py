@@ -29,6 +29,7 @@ from .native import (  # noqa: F401
     multi_gpu_decode_dump,
     shard_by_bytes,
     splitter_run,
+    splitter_run_capnp_framed,
     splitter_run_gelf,
     splitter_run_gelf_framed,
     splitter_run_ltsv_framed,

@@ -239,6 +239,10 @@ struct fg_ctx {
     std::vector<std::pair<std::string, std::string>> gelf_extra;
     Buf<uint8_t> ltsv_extra;   // output.ltsv_extra as the one literal the LTSV encoder writes (fg_set_ltsv_extra)
     int ltsv_extra_len = 0;
+    // output.capnp_extra (fg_set_capnp_extra): key 0, value 0, key 1, ... and their bounds [2n + 1], sorted by key
+    Buf<uint8_t> capnp_extra;
+    const int32_t* d_capnp_extra_off = nullptr;
+    int capnp_extra_n = 0;
     fg_out_framing out_framing = FG_OUT_NONE;  // output.framing of the fused encoder (fg_set_output_framing)
     // split mode (fg_split_decode)
     Buf<uint32_t> seg;
@@ -596,7 +600,11 @@ void begin_fused(fg_ctx* c, int fmt) {
 
 // The encoder a pipelined call runs after each parse step: none (the rows and side tables come back), or the GELF or
 // LTSV encoder (only the encoded records come back)
-enum Enc { ENC_NONE = 0, ENC_GELF = 1, ENC_LTSV = 2 };
+enum Enc { ENC_NONE = 0, ENC_GELF = 1, ENC_LTSV = 2, ENC_CAPNP = 3 };
+
+// the word of the counter block (past the K5_COUNT snapshotted ones) where the Cap'n Proto encoder reports the least
+// offset of a line whose record capnp cannot hold (0xFFFFFFFF: none)
+constexpr int kCapnpTooLong = 16;
 
 // The fused encoder `enc` over the decoder's results of lines [l0, l0 + n), parse step k
 int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, cudaStream_t s) {
@@ -620,7 +628,7 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
         E.gelf_entries = c->k.d + fg::K5_ENTRIES;
         // a line longer than the LTSV encoder's segment length field (2^29 - 1 bytes, the GELF encoder's is 2^30 - 1) may
         // hold a string with escapes that no segment holds: long_json_span_kernel looks for one
-        if (c->max_bytes >= ((size_t)1 << 29)) E.long_json_span = c->k.d + fg::K5_LONG_JSON_SPAN;
+        if (enc != ENC_CAPNP && c->max_bytes >= ((size_t)1 << 29)) E.long_json_span = c->k.d + fg::K5_LONG_JSON_SPAN;
     }
     if (fmt == FG_FMT_LTSV) {
         E.ltsv_suffix = c->ltsv.suffix;
@@ -639,9 +647,14 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
         E.static_key_off = c->d_static_key_off;
         E.static_lit_off = c->d_static_lit_off;
         E.static_kind = c->d_static_kind;
-    } else {
+    } else if (enc == ENC_LTSV) {
         E.static_blob = c->ltsv_extra.d;
         E.n_static = c->ltsv_extra_len;
+    } else {
+        E.static_blob = c->capnp_extra.d;
+        E.n_static = c->capnp_extra_n;
+        E.static_key_off = c->d_capnp_extra_off;
+        E.long_json_span = c->k.d + kCapnpTooLong;
     }
     E.lens = c->enc_lens.d + l0;
     E.rel = c->enc_rel.d + l0;
@@ -659,8 +672,9 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
     // the encoder's CTAs take 256 lines (4 x the parse kernel's 64); configure_gelf_encode allowed max_tile5
     E.tile_bytes = std::min(4 * tile, c->max_tile5);
     if (enc == ENC_GELF) FG_CUDA(c, fg::launch_gelf_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
-    else FG_CUDA(c, fg::launch_ltsv_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
-    c->launches += E.long_json_span ? 5 : 4;
+    else if (enc == ENC_LTSV) FG_CUDA(c, fg::launch_ltsv_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
+    else FG_CUDA(c, fg::launch_capnp_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
+    c->launches += E.long_json_span && enc != ENC_CAPNP ? 5 : 4;
     return FG_OK;
 }
 
@@ -1103,6 +1117,29 @@ int batch_lines(fg_ctx* c, int fmt, const uint8_t* bytes, const int32_t* offsets
     return fail(c, FG_E_CAPACITY, encode ? "output / side table overflow after regrow" : "side table overflow after regrow");
 }
 
+// The Cap'n Proto encoder's refusal of a record it cannot hold: reset before the call, read after it.  capnp-rust asserts
+// "Lists are limited to 2**29 elements" for a text of 2^29 - 1 bytes or more, so the reference writes no such message; the
+// call fails and its output is not handed out.
+int begin_capnp(fg_ctx* c, int enc) {
+    if (enc != ENC_CAPNP) return FG_OK;
+    FG_CUDA(c, cudaSetDevice(c->device));
+    FG_CUDA(c, cudaMemset(c->k.d + kCapnpTooLong, 0xFF, sizeof(uint32_t)));
+    return FG_OK;
+}
+
+// offsets [n + 1]: the batch's line offsets, which name the record the device reports by its first byte
+int end_capnp(fg_ctx* c, int enc, const int32_t* offsets, int32_t n) {
+    if (enc != ENC_CAPNP) return FG_OK;
+    uint32_t at = 0;
+    FG_CUDA(c, cudaMemcpy(&at, c->k.d + kCapnpTooLong, sizeof at, cudaMemcpyDeviceToHost));
+    if (at == 0xFFFFFFFFu) return FG_OK;
+    // the first line starting there that is not empty
+    int32_t line = (int32_t)(std::lower_bound(offsets, offsets + n, (int32_t)at) - offsets);
+    while (line + 1 < n && offsets[line + 1] == offsets[line]) ++line;
+    const std::string what = "record " + std::to_string(line) + ": a text of 2^29 - 1 bytes or more does not fit a Cap'n Proto message";
+    return fail(c, FG_E_ARG, what.c_str());
+}
+
 // decode + the encoder `enc` fused (fg_decode_encode_gelf / fg_decode_encode_ltsv)
 int decode_encode(fg_ctx* c, int enc, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
     if (!c || !out) return FG_E_ARG;
@@ -1111,7 +1148,9 @@ int decode_encode(fg_ctx* c, int enc, fg_format fmt, const uint8_t* bytes, const
     if (int rc = check_fusable(c, (int)fmt)) return rc;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;
+    if (int rc = begin_capnp(c, enc)) return rc;
     if (int rc = batch_lines(c, (int)fmt, bytes, offsets, n, enc, total, kms, tms)) return rc;
+    if (int rc = end_capnp(c, enc, offsets, n)) return rc;
     end_fused(c, (int)fmt, n, kms, tms, out);
     return FG_OK;
 }
@@ -1333,6 +1372,42 @@ int fg_set_ltsv_extra(fg_ctx* c, int32_t n, const char* const* keys, const char*
     return FG_OK;
 }
 
+// decode + CapnpEncoder::encode fused: the same pipeline with the Cap'n Proto encoder's kernels
+int fg_decode_encode_capnp(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
+    return decode_encode(c, ENC_CAPNP, fmt, bytes, offsets, n, out);
+}
+
+int fg_set_capnp_extra(fg_ctx* c, int32_t n, const char* const* keys, const char* const* values) {
+    if (!c || n < 0 || (n > 0 && (!keys || !values))) return FG_E_ARG;
+    std::vector<std::pair<std::string, std::string>> kv;
+    for (int32_t k = 0; k < n; ++k) {
+        if (!keys[k] || !values[k]) return fail(c, FG_E_ARG, "output.capnp_extra values must be strings");  // capnp_encoder.rs:25-27
+        kv.emplace_back(keys[k], values[k]);
+    }
+    std::sort(kv.begin(), kv.end());  // a TOML table iterates its keys in byte order
+    for (size_t k = 1; k < kv.size(); ++k)
+        if (kv[k].first == kv[k - 1].first) return fail(c, FG_E_ARG, "output.capnp_extra has a duplicate key");
+    FG_CUDA(c, cudaSetDevice(c->device));
+    FG_CUDA(c, cudaDeviceSynchronize());
+    // one blob: the bounds, then the text they index from the blob's start (the bounds take 2n + 1 words, padded to 16 bytes)
+    const int32_t text_at = (int32_t)((sizeof(int32_t) * (2 * kv.size() + 1) + 15) & ~(size_t)15);
+    std::string text;
+    std::vector<int32_t> off{text_at};
+    for (const auto& [k, v] : kv) {
+        text += k;
+        off.push_back(text_at + (int32_t)text.size());
+        text += v;
+        off.push_back(text_at + (int32_t)text.size());
+    }
+    Packer p;
+    p.add(off);
+    p.add(text);
+    if (int rc = p.upload(c, c->capnp_extra)) return rc;
+    c->d_capnp_extra_off = (const int32_t*)c->capnp_extra.d;
+    c->capnp_extra_n = (int)kv.size();
+    return FG_OK;
+}
+
 int fg_encoded_ltsv_stops(const fg_ctx* c, const int32_t** stop) {
     if (!c || !stop || c->enc_stop_n < 0) return FG_E_ARG;
     *stop = c->enc_stop.h;
@@ -1472,7 +1547,9 @@ int split_decode_encode(fg_ctx* c, int enc, fg_format fmt, fg_framing framing, c
     int32_t n;
     uint32_t total[fg::K5_COUNT];
     float kms, tms;
+    if (int rc = begin_capnp(c, enc)) return rc;
     if (int rc = split_stream(c, (int)fmt, framing, stream, nbytes, enc, n, total, kms, tms)) return rc;
+    if (int rc = end_capnp(c, enc, c->split_offsets.h, n)) return rc;
     end_fused(c, (int)fmt, n, kms, tms, out);
     *line_offsets = c->split_offsets.h;
     return FG_OK;
@@ -1512,6 +1589,12 @@ int fg_split_decode_encode_gelf(fg_ctx* c, fg_format fmt, fg_framing framing, co
 int fg_split_decode_encode_ltsv(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
                                 const int32_t** line_offsets) {
     return split_decode_encode(c, ENC_LTSV, fmt, framing, stream, nbytes, out, line_offsets);
+}
+
+// framing + decode + CapnpEncoder::encode on the device, as fg_split_decode_encode_gelf
+int fg_split_decode_encode_capnp(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
+                                 const int32_t** line_offsets) {
+    return split_decode_encode(c, ENC_CAPNP, fmt, framing, stream, nbytes, out, line_offsets);
 }
 
 int fg_upload(fg_ctx* c, const uint8_t* bytes, const int32_t* offsets, int32_t n) {

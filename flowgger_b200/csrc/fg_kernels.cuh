@@ -189,7 +189,8 @@ struct GelfEncodeParams {
     const uint32_t* gelf_entries;
     // GELF source, a context whose lines may pass 2^29 bytes: set by long_json_span_kernel when a span with JSON escapes
     // is longer than the encoder's segment length field holds (the call fails with FG_E_CAPACITY: such a span is not cut
-    // into segments); nullptr: the kernel is not launched
+    // into segments); nullptr: the kernel is not launched.  The Cap'n Proto encoder, which has no such kernel, takes the
+    // least offset in `bytes` of a line whose record capnp cannot hold here instead (atomicMin; 0xFFFFFFFF: none).
     uint32_t* long_json_span;
     // output.framing (fg_out_frame.cuh: OutFraming) applied to every record written
     int32_t out_framing;
@@ -204,6 +205,11 @@ size_t gelf_scan_temp_bytes(int n);
 // static_lit_off / static_kind arrays are unused.  The same scan temporary serves both.
 cudaError_t configure_ltsv_encode(int max_tile_bytes);
 cudaError_t launch_ltsv_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
+// ---- fused Cap'n Proto encoder over the same four decoders' results (fg_capnp_encode.cu) ------------------------------
+// The same parameters, except that static_blob holds output.capnp_extra as key 0, value 0, key 1, ... with n_static pairs
+// and static_key_off [2 n_static + 1] their bounds (sorted by key on the host); long_json_span receives the refusals.
+cudaError_t configure_capnp_encode(int max_tile_bytes);
+cudaError_t launch_capnp_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
 
 // RFC5424 (short lines, staged tile): 64-line CTAs — tile waits and barriers half as wide as with 128 lines
 #ifndef FG_R5_LINES  // other shapes build with -DFG_R5_LINES / -DFG_R5_MINB for A/B runs

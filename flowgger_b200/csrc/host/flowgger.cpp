@@ -225,21 +225,42 @@ void CudaBatchDecoder::decode_batch(const uint8_t* bytes, const int32_t* offsets
     if (rc != FG_OK) throw std::runtime_error(std::string("fg_decode_batch: ") + fg_last_error(ctx_));
 }
 
+namespace {
+// the C-ABI calls of each CudaFusedEncoder::Output, in its order
+struct FusedCalls {
+    const char* set_extra_name;
+    int (*set_extra)(fg_ctx*, int32_t, const char* const*, const char* const*);
+    const char* decode_encode_name;
+    int (*decode_encode)(fg_ctx*, fg_format, const uint8_t*, const int32_t*, int32_t, fg_encoded_out*);
+    const char* split_name;
+    int (*split)(fg_ctx*, fg_format, fg_framing, const uint8_t*, int64_t, fg_encoded_out*, const int32_t**);
+};
+const FusedCalls kFusedCalls[] = {
+    {"fg_set_gelf_extra: ", fg_set_gelf_extra, "fg_decode_encode_gelf: ", fg_decode_encode_gelf, "fg_split_decode_encode_gelf: ",
+     fg_split_decode_encode_gelf},
+    {"fg_set_ltsv_extra: ", fg_set_ltsv_extra, "fg_decode_encode_ltsv: ", fg_decode_encode_ltsv, "fg_split_decode_encode_ltsv: ",
+     fg_split_decode_encode_ltsv},
+    {"fg_set_capnp_extra: ", fg_set_capnp_extra, "fg_decode_encode_capnp: ", fg_decode_encode_capnp, "fg_split_decode_encode_capnp: ",
+     fg_split_decode_encode_capnp},
+};
+const FusedCalls& fused_calls(const CudaFusedEncoder& enc) { return kFusedCalls[(int)enc.output()]; }
+}  // namespace
+
 void CudaBatchDecoder::set_encoder(const CudaFusedEncoder& enc) {
     // set on every call: a host-side setting, and other callers of the same context may have changed it
     if (fg_set_output_framing(ctx_, enc.out_framing()) != FG_OK)
         throw std::runtime_error(std::string("fg_set_output_framing: ") + fg_last_error(ctx_));
     const std::vector<std::pair<std::string, std::string>>& extra = enc.extra();
-    const int o = enc.output() == CudaFusedEncoder::Output::Gelf ? 0 : 1;
+    const int o = (int)enc.output();
     if (extra_valid_[o] && extra == extra_set_[o]) return;
     std::vector<const char*> k, v;
     for (const auto& kv : extra) {
         k.push_back(kv.first.c_str());
         v.push_back(kv.second.c_str());
     }
-    const int rc = o == 0 ? fg_set_gelf_extra(ctx_, (int32_t)extra.size(), k.data(), v.data())
-                          : fg_set_ltsv_extra(ctx_, (int32_t)extra.size(), k.data(), v.data());
-    if (rc != FG_OK) throw std::runtime_error(std::string(o == 0 ? "fg_set_gelf_extra: " : "fg_set_ltsv_extra: ") + fg_last_error(ctx_));
+    const FusedCalls& f = fused_calls(enc);
+    if (f.set_extra(ctx_, (int32_t)extra.size(), k.data(), v.data()) != FG_OK)
+        throw std::runtime_error(std::string(f.set_extra_name) + fg_last_error(ctx_));
     extra_set_[o] = extra;
     extra_valid_[o] = true;
 }
@@ -253,10 +274,9 @@ void CudaBatchDecoder::decode_encode_gelf(const uint8_t* bytes, const int32_t* o
 void CudaBatchDecoder::decode_encode(const CudaFusedEncoder& enc, const uint8_t* bytes, const int32_t* offsets, int32_t n,
                                      fg_encoded_out* out) {
     set_encoder(enc);
-    const bool gelf = enc.output() == CudaFusedEncoder::Output::Gelf;
-    const int rc = (gelf ? fg_decode_encode_gelf : fg_decode_encode_ltsv)(ctx_, fmt_, bytes, offsets, n, out);
-    if (rc != FG_OK)
-        throw std::runtime_error(std::string(gelf ? "fg_decode_encode_gelf: " : "fg_decode_encode_ltsv: ") + fg_last_error(ctx_));
+    const FusedCalls& f = fused_calls(enc);
+    if (f.decode_encode(ctx_, fmt_, bytes, offsets, n, out) != FG_OK)
+        throw std::runtime_error(std::string(f.decode_encode_name) + fg_last_error(ctx_));
 }
 
 const int32_t* CudaBatchDecoder::encoded_ltsv_stops() const {
@@ -273,11 +293,10 @@ bool CudaBatchDecoder::try_split_decode_encode_gelf(const uint8_t* stream, int64
 bool CudaBatchDecoder::try_split_decode_encode(const CudaFusedEncoder& enc, const uint8_t* stream, int64_t nbytes, fg_framing framing,
                                                fg_encoded_out* out, const int32_t** line_offsets) {
     set_encoder(enc);
-    const bool gelf = enc.output() == CudaFusedEncoder::Output::Gelf;
-    const int rc = (gelf ? fg_split_decode_encode_gelf : fg_split_decode_encode_ltsv)(ctx_, fmt_, framing, stream, nbytes, out, line_offsets);
+    const FusedCalls& f = fused_calls(enc);
+    const int rc = f.split(ctx_, fmt_, framing, stream, nbytes, out, line_offsets);
     if (rc == FG_E_CAPACITY) return false;
-    if (rc != FG_OK)
-        throw std::runtime_error(std::string(gelf ? "fg_split_decode_encode_gelf: " : "fg_split_decode_encode_ltsv: ") + fg_last_error(ctx_));
+    if (rc != FG_OK) throw std::runtime_error(std::string(f.split_name) + fg_last_error(ctx_));
     return true;
 }
 
@@ -1254,6 +1273,21 @@ int fgh_splitter_run_ltsv_framed(void* d, const uint8_t* text, int64_t len, int3
     std::string stream, err, out;
     auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
     const CudaLtsvEncoder enc(extra_of(n_extra, keys, vals), (fg_out_framing)out_framing);
+    if (run_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
+    give(stream, out_stream, out_stream_len);
+    give(err, out_stderr, out_stderr_len);
+    give(out, out_stdout, out_stdout_len);
+    return 0;
+}
+
+// fgh_splitter_run_gelf_framed with output.format = "capnp" (CudaCapnpEncoder)
+int fgh_splitter_run_capnp_framed(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes, int n_extra,
+                                  const char* const* keys, const char* const* vals, int framing, int out_framing, uint8_t** out_stream,
+                                  int64_t* out_stream_len, uint8_t** out_stderr, int64_t* out_stderr_len, uint8_t** out_stdout,
+                                  int64_t* out_stdout_len) {
+    std::string stream, err, out;
+    auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
+    const CudaCapnpEncoder enc(extra_of(n_extra, keys, vals), (fg_out_framing)out_framing);
     if (run_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
     give(stream, out_stream, out_stream_len);
     give(err, out_stderr, out_stderr_len);

@@ -139,8 +139,8 @@ class CudaBatchDecoder {
     fg_format fmt_;
     fg_ctx* ctx_ = nullptr;
     std::mutex mu_;
-    std::vector<std::pair<std::string, std::string>> extra_set_[2];  // per CudaFusedEncoder::Output
-    bool extra_valid_[2] = {false, false};
+    std::vector<std::pair<std::string, std::string>> extra_set_[3];  // per CudaFusedEncoder::Output
+    bool extra_valid_[3] = {false, false, false};
     LtsvConfig ltsv_;
     DeviceOptions opt_;
     std::string suffix_[5];
@@ -200,20 +200,21 @@ class Encoder {
 // to run it on the device (CudaBatchDecoder::decode_encode / try_split_decode_encode).
 class CudaFusedEncoder : public Encoder {
    public:
-    enum class Output { Gelf, Ltsv };
+    enum class Output { Gelf, Ltsv, Capnp };
     // the decoders whose device-resident results the fused encoders read
     static bool fuses_with(fg_format fmt) {
         return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF;
     }
     // a lone host-side Record cannot be encoded: there is no CPU encoder behind this interface
     bool encode(Record&&, std::vector<uint8_t>&, const char** err) const override {
-        if (err)
-            *err = output_ == Output::Gelf ? "GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)"
-                                           : "LTSVEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)";
+        static const char* const kWhat[] = {"GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)",
+                                            "LTSVEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)",
+                                            "CapnpEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)"};
+        if (err) *err = kWhat[(int)output_];
         return false;
     }
     Output output() const { return output_; }
-    // output.gelf_extra or output.ltsv_extra
+    // output.gelf_extra, output.ltsv_extra or output.capnp_extra
     const std::vector<std::pair<std::string, std::string>>& extra() const { return extra_; }
     fg_out_framing out_framing() const { return out_framing_; }
 
@@ -240,6 +241,15 @@ class CudaLtsvEncoder : public CudaFusedEncoder {
    public:
     explicit CudaLtsvEncoder(std::vector<std::pair<std::string, std::string>> extra = {}, fg_out_framing out_framing = FG_OUT_NONE)
         : CudaFusedEncoder(Output::Ltsv, std::move(extra), out_framing) {}
+};
+
+// encoder/capnp_encoder.rs:14-45: output.format = "capnp", fused with the decoder on the GPU as CudaGelfEncoder is
+// (fg_decode_encode_capnp).  `extra` = output.capnp_extra (written in byte order of its keys), `out_framing` =
+// output.framing: FG_OUT_NONE is the reference's "noop" default for capnp (mod.rs:444-460).
+class CudaCapnpEncoder : public CudaFusedEncoder {
+   public:
+    explicit CudaCapnpEncoder(std::vector<std::pair<std::string, std::string>> extra = {}, fg_out_framing out_framing = FG_OUT_NONE)
+        : CudaFusedEncoder(Output::Capnp, std::move(extra), out_framing) {}
 };
 
 // What RecordBatcher and the batching splitters do with each record of a batch decoded on the device, one record at a

@@ -110,6 +110,9 @@ def load_cuda() -> C.CDLL:
         L.fg_set_ltsv_extra.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_char_p)]
         L.fg_decode_encode_ltsv.argtypes = L.fg_decode_encode_gelf.argtypes
         L.fg_split_decode_encode_ltsv.argtypes = L.fg_split_decode_encode_gelf.argtypes
+        L.fg_set_capnp_extra.argtypes = L.fg_set_ltsv_extra.argtypes
+        L.fg_decode_encode_capnp.argtypes = L.fg_decode_encode_gelf.argtypes
+        L.fg_split_decode_encode_capnp.argtypes = L.fg_split_decode_encode_gelf.argtypes
         L.fg_encoded_ltsv_stops.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
         L.fg_encoded_gelf_now.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         L.fg_set_output_framing.argtypes = [C.c_void_p, C.c_int]
@@ -152,6 +155,7 @@ def load_host() -> C.CDLL:
         L.fgh_splitter_run_gelf_framed.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int64, C.c_int, C.POINTER(C.c_char_p),
                                                    C.POINTER(C.c_char_p), C.c_int, C.c_int] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         L.fgh_splitter_run_ltsv_framed.argtypes = L.fgh_splitter_run_gelf_framed.argtypes
+        L.fgh_splitter_run_capnp_framed.argtypes = L.fgh_splitter_run_gelf_framed.argtypes
         L.fgh_splitter_run.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int64, C.c_int32, C.c_int64] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         _host = L
     return _host
@@ -437,6 +441,21 @@ class BatchDecoder:
         """split_decode_encode_gelf with the LTSV encoder (fg_split_decode_encode_ltsv)."""
         return self._split_decode_encode("fg_split_decode_encode_ltsv", stream, framing, copy)
 
+    def set_capnp_extra(self, extra: dict[str, str]) -> None:
+        """output.capnp_extra of CapnpEncoder::new (capnp_encoder.rs:14-32); written in byte order of the keys."""
+        self._check(self.L.fg_set_capnp_extra(self.ctx, *_extra_arrays(extra)), "fg_set_capnp_extra")
+
+    def decode_encode_capnp(self, data: np.ndarray, offsets: np.ndarray, copy: bool = True):
+        """decode + CapnpEncoder::encode fused on the device (fg_decode_encode_capnp), for the same four decoders as
+        decode_encode_gelf and with the same results: (Cap'n Proto bytes, int64 offsets[n+1], status uint8[n], kernel ms).
+        A record is the serialized message of record.capnp's Record: the segment table, then the segments' words.  The
+        default output.framing of capnp is none ("noop")."""
+        return self._decode_encode("fg_decode_encode_capnp", data, offsets, copy)
+
+    def split_decode_encode_capnp(self, stream: np.ndarray, framing: int = 0, copy: bool = True):
+        """split_decode_encode_gelf with the Cap'n Proto encoder (fg_split_decode_encode_capnp)."""
+        return self._split_decode_encode("fg_split_decode_encode_capnp", stream, framing, copy)
+
     def _decode_encode(self, fn: str, data: np.ndarray, offsets: np.ndarray, copy: bool):
         assert data.dtype == np.uint8 and offsets.dtype == np.int32
         out = FgEncodedOut()
@@ -651,6 +670,17 @@ def splitter_run_ltsv_framed(dec: "BatchDecoder", text: bytes, out_framing: int,
     n_extra, keys, vals = _extra_arrays(extra)
     return _run_splitter(lambda o: H.fgh_splitter_run_ltsv_framed(dec._h, text, len(text), max_lines, max_bytes, n_extra, keys,
                                                                   vals, framing, out_framing, *o))
+
+
+def splitter_run_capnp_framed(dec: "BatchDecoder", text: bytes, out_framing: int = 0, extra: dict[str, str] | None = None,
+                              max_lines: int = 1 << 16, max_bytes: int = 16 << 20, framing: int = 0) -> tuple[bytes, bytes, bytes]:
+    """splitter_run_gelf_framed with output.format = "capnp" (CudaCapnpEncoder, output.capnp_extra = extra; output.framing
+    defaults to none, the reference's "noop" for capnp): returns (the output stream exactly as the splitter sent it, stderr
+    text, stdout text)."""
+    H = load_host()
+    n_extra, keys, vals = _extra_arrays(extra)
+    return _run_splitter(lambda o: H.fgh_splitter_run_capnp_framed(dec._h, text, len(text), max_lines, max_bytes, n_extra, keys,
+                                                                   vals, framing, out_framing, *o))
 
 
 def splitter_run(dec: "BatchDecoder", text: bytes, max_lines: int = 1 << 16, max_bytes: int = 16 << 20,

@@ -329,6 +329,27 @@ int fg_decode_encode_ltsv(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_
                           const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
 int fg_split_decode_encode_ltsv(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */, fg_framing framing,
                                 const uint8_t* stream, int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
+/* output.format = "capnp" (encoder/capnp_encoder.rs:14-109, record.capnp), the same four input formats:
+ *     CapnpEncoder::new(&Config)  capnp_encoder.rs:14-32   -> fg_set_capnp_extra (output.capnp_extra)
+ *     Encoder::encode(Record)     capnp_encoder.rs:36-45   -> fg_decode_encode_capnp / fg_split_decode_encode_capnp
+ * Record i is the message capnp::serialize::write_message writes for build_record's Record (capnp 0.14, a default
+ * Builder): the segment table, then each segment's words.  Record = ts (f64), facility and severity (u8, 255 = None),
+ * and the texts hostname, appname, procid, msgid, msg, fullMsg where the Record has them; of the FIRST SD element only,
+ * sdId (RFC5424) and its pairs (key '_' + name, for LTSV input + the type suffix; string values as text, bool / f64 / i64
+ * / u64 / null as the union's member); output.capnp_extra as the `extra` pairs, keys as given.  No byte is escaped; a
+ * GELF string is its unescaped text.  A record up to 8 KiB or so is one segment; a longer one takes more, as capnp-rust's
+ * HeapAllocator places them.  The reference writes no message holding a text of 2^29 - 1 bytes or more (capnp-rust
+ * asserts): such a line fails the call with FG_E_ARG and a text naming the record, and no output is handed out.
+ * Everything else — fg_encoded_out, statuses, empty rejected records, output.framing (the caller resolves the
+ * reference's "noop" default for capnp: FG_OUT_NONE), fg_encoded_ltsv_stops, fg_encoded_gelf_now, FG_E_CAPACITY, the
+ * input format rule — is exactly as for the GELF twins above.
+ * fg_set_capnp_extra: the extras are written in byte order of their keys (a TOML table); a duplicate key or a NULL
+ * string -> FG_E_ARG with the extras unchanged; n = 0 clears them. */
+int fg_set_capnp_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
+int fg_decode_encode_capnp(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */,
+                           const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
+int fg_split_decode_encode_capnp(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */, fg_framing framing,
+                                 const uint8_t* stream, int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
 /* The one side effect of LTSVDecoder::decode, println!("Missing value for name '{}'") for every tab-separated part
  * without ':' that the decode loop reached (ltsv_decoder.rs:99), for the records of the last fused call on an LTSV
  * context.  *stop ([out->n], valid until the next call on the context): -1 when record i printed nothing; else the offset,

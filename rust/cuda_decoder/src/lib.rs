@@ -46,7 +46,7 @@ struct Ctx {
     suffix: [Option<String>; 5],
     spec: CtxSpec,
     max_bytes: usize,                        // max_batch_bytes as fg_create took it
-    extra: [Option<Vec<(String, String)>>; 2],  // the output.gelf_extra / output.ltsv_extra last set on the context
+    extra: [Option<Vec<(String, String)>>; 3],  // the output.gelf_extra / ltsv_extra / capnp_extra last set on the context
 }
 unsafe impl Send for Ctx {}
 impl Drop for Ctx {
@@ -139,7 +139,7 @@ impl CudaDecoder {
         }
         let max_bytes = if max_bytes > 0 { (max_bytes as usize).min(0x7FFF_FFC0) } else { 256 << 20 };  // fg_create's default and cap
         let suffix = spec.suffix.clone();
-        CudaDecoder { ctx: Arc::new(Mutex::new(Ctx { raw, fmt, suffix, spec, max_bytes, extra: [None, None] })) }
+        CudaDecoder { ctx: Arc::new(Mutex::new(Ctx { raw, fmt, suffix, spec, max_bytes, extra: [None, None, None] })) }
     }
 
     /// max_batch_bytes of the context
@@ -227,9 +227,10 @@ impl CudaDecoder {
         self.split_decode_encode(FusedOutput::Gelf, stream, extra, out_framing, f, all)
     }
 
-    /// `split_decode_encode_gelf` for either fused encoder: `output` = output.format, `extra` = its extras
-    /// (output.gelf_extra or output.ltsv_extra); with `FusedOutput::Ltsv` the records are `LTSVEncoder::encode`'s text
-    /// (`fg_split_decode_encode_ltsv`).
+    /// `split_decode_encode_gelf` for any fused encoder: `output` = output.format, `extra` = its extras
+    /// (output.gelf_extra, output.ltsv_extra or output.capnp_extra); with `FusedOutput::Ltsv` the records are
+    /// `LTSVEncoder::encode`'s text (`fg_split_decode_encode_ltsv`), with `FusedOutput::Capnp` `CapnpEncoder::encode`'s
+    /// messages (`fg_split_decode_encode_capnp`).
     pub fn split_decode_encode<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String]), G: FnOnce(&[u8])>(
         &self, output: FusedOutput, stream: &[u8], extra: &[(String, String)], out_framing: fg_out_framing, mut f: F, all: G) -> bool {
         let mut ctx = self.ctx.lock().unwrap();
@@ -240,13 +241,21 @@ impl CudaDecoder {
             let vals: Vec<CString> = extra.iter().map(|(_, v)| CString::new(v.as_str()).unwrap()).collect();
             let kp: Vec<*const c_char> = keys.iter().map(|s| s.as_ptr()).collect();
             let vp: Vec<*const c_char> = vals.iter().map(|s| s.as_ptr()).collect();
-            let set = match output { FusedOutput::Gelf => fg_set_gelf_extra, FusedOutput::Ltsv => fg_set_ltsv_extra };
+            let set = match output {
+                FusedOutput::Gelf => fg_set_gelf_extra,
+                FusedOutput::Ltsv => fg_set_ltsv_extra,
+                FusedOutput::Capnp => fg_set_capnp_extra,
+            };
             assert_eq!(unsafe { set(ctx.raw, kp.len() as i32, kp.as_ptr(), vp.as_ptr()) }, 0);
             ctx.extra[o] = Some(extra.to_vec());
         }
         let mut out: fg_encoded_out = unsafe { std::mem::zeroed() };
         let mut lines: *const i32 = ptr::null();
-        let call = match output { FusedOutput::Gelf => fg_split_decode_encode_gelf, FusedOutput::Ltsv => fg_split_decode_encode_ltsv };
+        let call = match output {
+            FusedOutput::Gelf => fg_split_decode_encode_gelf,
+            FusedOutput::Ltsv => fg_split_decode_encode_ltsv,
+            FusedOutput::Capnp => fg_split_decode_encode_capnp,
+        };
         let rc = unsafe { call(ctx.raw, ctx.fmt, fg_framing_FG_FRAME_LINE, stream.as_ptr(), stream.len() as i64, &mut out, &mut lines) };
         if rc == FG_E_CAPACITY {
             return false;
@@ -603,11 +612,19 @@ pub fn fuses_with_ltsv(input_format: &str) -> bool {
     fuses_with_gelf(input_format)
 }
 
-/// The output format of a fused encoder (output.format = "gelf" or "ltsv")
+/// The `input.format` values whose decoder runs fused with the Cap'n Proto encoder on the device
+/// (`fg_decode_encode_capnp`, `fg_split_decode_encode_capnp`): the same four; `FusedCapnpLineSplitter` takes a
+/// `CudaDecoder` of one of them.
+pub fn fuses_with_capnp(input_format: &str) -> bool {
+    fuses_with_gelf(input_format)
+}
+
+/// The output format of a fused encoder (output.format = "gelf", "ltsv" or "capnp")
 #[derive(Clone, Copy, PartialEq, Eq, Debug)]
 pub enum FusedOutput {
     Gelf = 0,
     Ltsv = 1,
+    Capnp = 2,
 }
 
 /// The device framing of an `output.framing` value, as `mod.rs:453-460` picks the merger (panics on an unknown one, as
@@ -657,6 +674,22 @@ pub struct FusedLtsvLineSplitter {
 impl<T: Read> Splitter<T> for FusedLtsvLineSplitter {
     fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
         run_fused(&self.gpu, FusedOutput::Ltsv, &self.extra, self.out_framing, self.max_bytes, buf_reader, tx)
+    }
+}
+
+/// `output.format = "capnp"` with `input.format` one of `fuses_with_capnp`: `FusedGelfLineSplitter` with the Cap'n Proto
+/// encoder (`fg_split_decode_encode_capnp`, replaces Decoder::decode + CapnpEncoder::encode, capnp_encoder.rs:36-109).
+/// The caller resolves output.framing's default, "noop" for capnp (mod.rs:444-460): `FG_OUT_NONE`, one `Vec` per record.
+pub struct FusedCapnpLineSplitter {
+    pub gpu: CudaDecoder,
+    pub extra: Vec<(String, String)>,   // output.capnp_extra (capnp_encoder.rs:14-32), in byte order of the keys
+    pub out_framing: fg_out_framing,    // output.framing (mod.rs:444-460), resolved by the caller
+    pub max_bytes: usize,
+}
+
+impl<T: Read> Splitter<T> for FusedCapnpLineSplitter {
+    fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
+        run_fused(&self.gpu, FusedOutput::Capnp, &self.extra, self.out_framing, self.max_bytes, buf_reader, tx)
     }
 }
 
