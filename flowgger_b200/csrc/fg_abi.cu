@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "../../include/flowgger_cuda.h"
+#include "fg_capnp_layout.cuh"
 #include "fg_kernels.cuh"
 #include "fg_status.h"
 #include "fg_rfc3164.cuh"
@@ -1379,25 +1380,33 @@ int fg_decode_encode_capnp(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const
 
 int fg_set_capnp_extra(fg_ctx* c, int32_t n, const char* const* keys, const char* const* values) {
     if (!c || n < 0 || (n > 0 && (!keys || !values))) return FG_E_ARG;
-    std::vector<std::pair<std::string, std::string>> kv;
+    // A key or value of 2^29 - 1 bytes or more is a text capnp-rust asserts on in every record; the blob's bounds are
+    // int32: both are refused here, before anything is copied, and the extras in use stay.
+    const size_t text_at = (sizeof(int32_t) * (2 * (size_t)n + 1) + 15) & ~(size_t)15;
+    size_t total = text_at;
     for (int32_t k = 0; k < n; ++k) {
         if (!keys[k] || !values[k]) return fail(c, FG_E_ARG, "output.capnp_extra values must be strings");  // capnp_encoder.rs:25-27
-        kv.emplace_back(keys[k], values[k]);
+        const size_t kl = strlen(keys[k]), vl = strlen(values[k]);
+        if (kl + 1 >= fg::kCapMaxWords || vl + 1 >= fg::kCapMaxWords)
+            return fail(c, FG_E_ARG, "output.capnp_extra: a key or value of 2^29 - 1 bytes or more does not fit a Cap'n Proto message");
+        total += kl + vl;
+        if (total > (size_t)INT32_MAX) return fail(c, FG_E_ARG, "output.capnp_extra: more than 2^31 - 1 bytes in all");
     }
+    std::vector<std::pair<std::string, std::string>> kv;
+    for (int32_t k = 0; k < n; ++k) kv.emplace_back(keys[k], values[k]);
     std::sort(kv.begin(), kv.end());  // a TOML table iterates its keys in byte order
     for (size_t k = 1; k < kv.size(); ++k)
         if (kv[k].first == kv[k - 1].first) return fail(c, FG_E_ARG, "output.capnp_extra has a duplicate key");
     FG_CUDA(c, cudaSetDevice(c->device));
     FG_CUDA(c, cudaDeviceSynchronize());
     // one blob: the bounds, then the text they index from the blob's start (the bounds take 2n + 1 words, padded to 16 bytes)
-    const int32_t text_at = (int32_t)((sizeof(int32_t) * (2 * kv.size() + 1) + 15) & ~(size_t)15);
     std::string text;
-    std::vector<int32_t> off{text_at};
+    std::vector<int32_t> off{(int32_t)text_at};
     for (const auto& [k, v] : kv) {
         text += k;
-        off.push_back(text_at + (int32_t)text.size());
+        off.push_back((int32_t)(text_at + text.size()));
         text += v;
-        off.push_back(text_at + (int32_t)text.size());
+        off.push_back((int32_t)(text_at + text.size()));
     }
     Packer p;
     p.add(off);

@@ -26,10 +26,11 @@ namespace fg {
 
 namespace {
 
-// the kind of a segment, in bits 29..31 of its length
+// the kind of a segment, read from its 32-bit length word: 0 is a NUL and pad (CK_END), all ones a computed word
+// (CK_WORD), bit 31 a GELF span with JSON escapes (CK_JSON), else raw bytes.  A span holds less than 2^31 bytes, so a
+// length holds any span a line can hold, also the raw JSON of a GELF string whose unescaped text capnp holds.
 enum : uint32_t { CK_WORD = 0, CK_RAW = 1, CK_JSON = 2, CK_END = 3 };
-constexpr int kKindShift = 29;
-constexpr uint32_t kLenMask = (1u << kKindShift) - 1u;
+constexpr uint32_t kLenEnd = 0u, kLenWord = 0xFFFFFFFFu, kLenJson = 1u << 31;
 
 __device__ const uint8_t kUnderscore[] = "_";
 
@@ -45,17 +46,18 @@ struct CapSegs {
     __device__ __forceinline__ bool full() const { return n == kMaxCapSegs; }
     // the next `k` segments all lie before the window
     __device__ __forceinline__ bool before(unsigned long long k) const { return idx + k <= (unsigned long long)skip; }
-    __device__ __forceinline__ void push(const uint8_t* q, uint32_t l, uint32_t kind) {
+    // l: a length word (kLenEnd, kLenWord, or a span's length, | kLenJson for one with escapes)
+    __device__ __forceinline__ void push(const uint8_t* q, uint32_t l) {
         if (idx >= skip && n < kMaxCapSegs) {
             p[n] = q;
-            len[n] = l | (kind << kKindShift);
+            len[n] = l;
             ++n;
         }
         ++idx;
     }
-    __device__ __forceinline__ void word(unsigned long long v) { push(reinterpret_cast<const uint8_t*>(v), 8u, CK_WORD); }
+    __device__ __forceinline__ void word(unsigned long long v) { push(reinterpret_cast<const uint8_t*>(v), kLenWord); }
     __device__ __forceinline__ void bytes(Span s, bool json) {
-        if (s.len > 0) push(s.p, (uint32_t)s.len, json ? CK_JSON : CK_RAW);
+        if (s.len > 0) push(s.p, (uint32_t)s.len | (json ? kLenJson : 0u));
     }
 };
 
@@ -84,11 +86,9 @@ __device__ __forceinline__ uint32_t span_text_len(Span s, bool esc, bool mode2) 
 __device__ __forceinline__ uint32_t text_len(const CapText& t, bool mode2) {
     return (t.us ? 1u : 0u) + span_text_len(t.body, t.esc, mode2) + (uint32_t)t.suffix.len;
 }
-// capnp holds a text of len bytes (its NUL included, a list of under 2^29 bytes); a segment's length field holds the
-// body, which for a GELF string with escapes is longer than its text
-__device__ __forceinline__ bool text_fits(const CapText& t, uint32_t len) {
-    return len + 1u < kCapMaxWords && (uint32_t)t.body.len <= kLenMask;
-}
+// capnp holds a text of len bytes: its NUL included, a list of under 2^29 bytes.  Only the text counts: the span of a
+// GELF string with escapes, longer than its text, has a segment length of its own.
+__device__ __forceinline__ bool text_fits(uint32_t len) { return len + 1u < kCapMaxWords; }
 
 struct CapRec {
     CapText f[CP_SDID + 1];
@@ -213,7 +213,7 @@ __device__ __forceinline__ bool place_all(const GelfEncodeParams& P, const ByteS
     A.place(0, kCapRootWords);
     for (int k = 0; k <= CP_SDID; ++k) {
         if (!((c.fmask >> k) & 1u)) continue;
-        ok = ok && text_fits(c.f[k], c.flen[k]);
+        ok = ok && text_fits(c.flen[k]);
         const CapPlace pl = A.place(0, cap_text_words(c.flen[k]));
         if (kids) kids[k] = pl;
     }
@@ -228,11 +228,11 @@ __device__ __forceinline__ bool place_all(const GelfEncodeParams& P, const ByteS
             CapPair q;
             any_pair<Src>(P, B, r, extra, extra ? j : c.pa + j, q);
             const uint32_t kl = text_len(q.key, c.mode2);
-            ok = ok && text_fits(q.key, kl);
+            ok = ok && text_fits(kl);
             A.place(pl.seg, cap_text_words(kl));
             if (q.tag == 0u) {
                 const uint32_t vl = text_len(q.val, c.mode2);
-                ok = ok && text_fits(q.val, vl);
+                ok = ok && text_fits(vl);
                 A.place(pl.seg, cap_text_words(vl));
             }
         }
@@ -245,10 +245,10 @@ __device__ __forceinline__ void pad_if_far(CapSegs& L, const CapPlace& pl, uint3
     if (pl.pad >= 0) L.word(cap_pad_word(kind, hi));
 }
 __device__ __forceinline__ void push_text(CapSegs& L, const CapText& t) {
-    if (t.us) L.push(kUnderscore, 1u, CK_RAW);
+    if (t.us) L.push(kUnderscore, 1u);
     L.bytes(t.body, t.esc);
     L.bytes(t.suffix, false);
-    L.push(nullptr, 0u, CK_END);
+    L.push(nullptr, kLenEnd);
 }
 
 // The segments of window L (from L.skip on, up to kMaxCapSegs of them): the segment table, then the words of each
@@ -349,9 +349,9 @@ __device__ __forceinline__ void run_capnp(const CapSegs& L, bool live, Sink& s, 
     bool more = live && L.n > 0;
     auto enter = [&](int j) {
         p = L.p[j];
-        kind = L.len[j] >> kKindShift;
-        len = (int)(L.len[j] & kLenMask);
-        if (kind == CK_END) len = 8 - (int)(done & 7u);
+        const uint32_t l = L.len[j];
+        kind = l == kLenWord ? CK_WORD : l == kLenEnd ? CK_END : (l & kLenJson) ? CK_JSON : CK_RAW;
+        len = kind == CK_WORD ? 8 : kind == CK_END ? 8 - (int)(done & 7u) : (int)(l & ~kLenJson);
         k = 0;
     };
     if (more) enter(0);

@@ -343,8 +343,9 @@ int fg_split_decode_encode_ltsv(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | F
  * Everything else — fg_encoded_out, statuses, empty rejected records, output.framing (the caller resolves the
  * reference's "noop" default for capnp: FG_OUT_NONE), fg_encoded_ltsv_stops, fg_encoded_gelf_now, FG_E_CAPACITY, the
  * input format rule — is exactly as for the GELF twins above.
- * fg_set_capnp_extra: the extras are written in byte order of their keys (a TOML table); a duplicate key or a NULL
- * string -> FG_E_ARG with the extras unchanged; n = 0 clears them. */
+ * fg_set_capnp_extra: the extras are written in byte order of their keys (a TOML table); a duplicate key, a NULL
+ * string, a key or value of 2^29 - 1 bytes or more (no record could hold it) or more than 2^31 - 1 bytes of keys and
+ * values in all -> FG_E_ARG with the extras unchanged; n = 0 clears them. */
 int fg_set_capnp_extra(fg_ctx* ctx, int32_t n, const char* const* keys, const char* const* values);
 int fg_decode_encode_capnp(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */,
                            const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);

@@ -3,7 +3,9 @@ with g++ by tests/emu/emu_capnp.cpp) place every object of a message where the r
 does and point to it with the same words, and the restated encoder is pinned to the reference's three tests and read
 back by the wire-format reader.  Records cover the NUL / pad boundary of texts, messages of 1022..1026 words, objects
 that back-fill segment 0 after a large one went to a new segment, extras across the segment boundary, 0, 1 and 1000
-pairs and every union member.  No GPU needed."""
+pairs and every union member.  The model of the encoder's segment list (tests/capnp_out_edges.py) joins to the
+oracle's message on the random records and on every window line, whose coverage of the window boundaries is checked
+here.  No GPU needed."""
 import ctypes as C
 import json
 import random
@@ -15,6 +17,7 @@ import numpy as np
 import pytest
 
 import capnp_oracle as O
+import capnp_out_edges as CE
 
 HERE = Path(__file__).resolve().parent
 
@@ -164,3 +167,45 @@ def test_random_multi_segment(emu):
         rec = record(host=txt(), app=txt() if rng.random() < 0.5 else None, msg=txt(), full=txt(),
                      sd=[(txt() if rng.random() < 0.5 else None, pairs)] if pairs or rng.random() < 0.3 else None)
         check_layout(emu, rec, [(b"x%d" % j, txt()) for j in range(rng.choice([0, 0, 2, 5]))])
+
+
+# ---- the segment list model of tests/capnp_out_edges.py ---------------------------------------------------------------
+
+def test_segment_model_random_records():
+    """the model's entries, joined, are the oracle's message for the 300 random multi-segment records"""
+    rng = random.Random(7)
+    for _ in range(300):
+        def txt():
+            return b"t" * rng.choice([0, 1, 7, 8, 100, 3000, 9000, 20000, 70000])
+        pairs = [(b"_" + txt(), ("string", txt()) if rng.random() < 0.7 else ("u64", rng.getrandbits(64)))
+                 for _ in range(rng.choice([0, 1, 3, 40]))]
+        rec = record(host=txt(), app=txt() if rng.random() < 0.5 else None, msg=txt(), full=txt(),
+                     sd=[(txt() if rng.random() < 0.5 else None, pairs)] if pairs or rng.random() < 0.3 else None)
+        extra = [(b"x%d" % j, txt()) for j in range(rng.choice([0, 0, 2, 5]))]
+        assert b"".join(b for _, b in CE.segments(rec, extra)) == O.encode(rec, extra)
+
+
+@pytest.mark.parametrize("src", [CE.R5, CE.LTSV, CE.GELF, CE.R3])
+def test_window_lines_model(oracle, src):
+    """every window line's record: the model joins to the oracle's message, and the lines reach every (boundary, kind)
+    cell, every total and every after-a-list cell they claim, with and without extras"""
+    lines = CE.window_lines(src)
+    cfg = oracle.LtsvConfig(CE.TYPED, CE.SUFFIXES) if src == CE.LTSV else oracle.Rfc3164Config(2026) if src == CE.R3 else None
+    recs = O.decode_records(oracle, src, *oracle.pack(lines), cfg=cfg)
+    assert all(r is not None for r in recs)
+    cells, totals, after = set(), set(), set()
+    for extra in ([], O.extra_pairs(CE.EXTRA)):
+        for r in recs:
+            assert b"".join(b for _, b in CE.segments(r, extra, src)) == O.encode(r, extra)
+            c, t, a = CE.cells(r, extra, src)
+            cells, after = cells | c, after | a
+            totals.add(t)
+    assert not {(b, k) for b in CE.BOUNDARIES for k in CE.KINDS[src]} - cells
+    assert not CE.AFTER_LIST[src] - after
+    if src != CE.R3:
+        assert set(CE.TOTALS) <= totals
+    if src != CE.R3:  # lane_lines' records end on the window boundaries or take four windows
+        shapes = CE.LANE_SHAPES[src]
+        got = [len(CE.segments(r, [], src)) for r in O.decode_records(
+            oracle, src, *oracle.pack([CE.lane_line(src, *shapes[k]) for k in (64, 128, 4)]), cfg=cfg)]
+        assert got[:2] == [64, 128] and 192 < got[2] <= 256
