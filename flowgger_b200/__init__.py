@@ -33,6 +33,7 @@ from .native import (  # noqa: F401
     splitter_run_gelf,
     splitter_run_gelf_framed,
     splitter_run_ltsv_framed,
+    splitter_run_passthrough_framed,
     tz_count,
     tz_lookup,
 )

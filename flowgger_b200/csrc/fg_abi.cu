@@ -244,6 +244,9 @@ struct fg_ctx {
     Buf<uint8_t> capnp_extra;
     const int32_t* d_capnp_extra_off = nullptr;
     int capnp_extra_n = 0;
+    // the header of every passthrough record (fg_set_passthrough_prefix)
+    Buf<uint8_t> pt_prefix;
+    int32_t pt_prefix_len = 0;
     fg_out_framing out_framing = FG_OUT_NONE;  // output.framing of the fused encoder (fg_set_output_framing)
     // split mode (fg_split_decode)
     Buf<uint32_t> seg;
@@ -599,9 +602,9 @@ void begin_fused(fg_ctx* c, int fmt) {
     c->gelf_now = (double)t.tv_sec + (double)t.tv_nsec / 1e9;
 }
 
-// The encoder a pipelined call runs after each parse step: none (the rows and side tables come back), or the GELF or
-// LTSV encoder (only the encoded records come back)
-enum Enc { ENC_NONE = 0, ENC_GELF = 1, ENC_LTSV = 2, ENC_CAPNP = 3 };
+// The encoder a pipelined call runs after each parse step: none (the rows and side tables come back), or the GELF, LTSV,
+// Cap'n Proto or passthrough encoder (only the encoded records come back)
+enum Enc { ENC_NONE = 0, ENC_GELF = 1, ENC_LTSV = 2, ENC_CAPNP = 3, ENC_PASSTHROUGH = 4 };
 
 // the word of the counter block (past the K5_COUNT snapshotted ones) where the Cap'n Proto encoder reports the least
 // offset of a line whose record capnp cannot hold (0xFFFFFFFF: none)
@@ -628,8 +631,9 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
         E.gelf_now = c->gelf_now;
         E.gelf_entries = c->k.d + fg::K5_ENTRIES;
         // a line longer than the LTSV encoder's segment length field (2^29 - 1 bytes, the GELF encoder's is 2^30 - 1) may
-        // hold a string with escapes that no segment holds: long_json_span_kernel looks for one
-        if (enc != ENC_CAPNP && c->max_bytes >= ((size_t)1 << 29)) E.long_json_span = c->k.d + fg::K5_LONG_JSON_SPAN;
+        // hold a string with escapes that no segment holds: long_json_span_kernel looks for one.  The passthrough
+        // encoder has no segment length field.
+        if ((enc == ENC_GELF || enc == ENC_LTSV) && c->max_bytes >= ((size_t)1 << 29)) E.long_json_span = c->k.d + fg::K5_LONG_JSON_SPAN;
     }
     if (fmt == FG_FMT_LTSV) {
         E.ltsv_suffix = c->ltsv.suffix;
@@ -651,11 +655,14 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
     } else if (enc == ENC_LTSV) {
         E.static_blob = c->ltsv_extra.d;
         E.n_static = c->ltsv_extra_len;
-    } else {
+    } else if (enc == ENC_CAPNP) {
         E.static_blob = c->capnp_extra.d;
         E.n_static = c->capnp_extra_n;
         E.static_key_off = c->d_capnp_extra_off;
         E.long_json_span = c->k.d + kCapnpTooLong;
+    } else {
+        E.static_blob = c->pt_prefix.d;
+        E.n_static = c->pt_prefix_len;
     }
     E.lens = c->enc_lens.d + l0;
     E.rel = c->enc_rel.d + l0;
@@ -674,7 +681,8 @@ int launch_encode(fg_ctx* c, int enc, int fmt, int k, int l0, int n, int tile, c
     E.tile_bytes = std::min(4 * tile, c->max_tile5);
     if (enc == ENC_GELF) FG_CUDA(c, fg::launch_gelf_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
     else if (enc == ENC_LTSV) FG_CUDA(c, fg::launch_ltsv_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
-    else FG_CUDA(c, fg::launch_capnp_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
+    else if (enc == ENC_CAPNP) FG_CUDA(c, fg::launch_capnp_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
+    else FG_CUDA(c, fg::launch_passthrough_encode(fmt, E, c->scan_temp.d, c->scan_temp_bytes, s));
     c->launches += E.long_json_span && enc != ENC_CAPNP ? 5 : 4;
     return FG_OK;
 }
@@ -1417,6 +1425,25 @@ int fg_set_capnp_extra(fg_ctx* c, int32_t n, const char* const* keys, const char
     return FG_OK;
 }
 
+// decode + PassthroughEncoder::encode fused: the same pipeline with the passthrough encoder's kernels
+int fg_decode_encode_passthrough(fg_ctx* c, fg_format fmt, const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out) {
+    return decode_encode(c, ENC_PASSTHROUGH, fmt, bytes, offsets, n, out);
+}
+
+int fg_set_passthrough_prefix(fg_ctx* c, const uint8_t* bytes, int64_t n) {
+    if (!c || n < 0) return FG_E_ARG;
+    if (n > 0 && !bytes) return fail(c, FG_E_ARG, "passthrough prefix: NULL bytes");
+    if (n > (int64_t)INT32_MAX) return fail(c, FG_E_ARG, "passthrough prefix: 2^31 bytes or more");
+    FG_CUDA(c, cudaSetDevice(c->device));
+    FG_CUDA(c, cudaDeviceSynchronize());
+    c->pt_prefix_len = 0;
+    // set once per call by the host layers (the header carries the time): the buffer is kept while the header fits
+    if (c->pt_prefix.n < (size_t)n + 16) FG_CUDA(c, c->pt_prefix.alloc((size_t)n + 16, DEV));
+    if (n > 0) FG_CUDA(c, cudaMemcpy(c->pt_prefix.d, bytes, (size_t)n, cudaMemcpyHostToDevice));
+    c->pt_prefix_len = (int32_t)n;
+    return FG_OK;
+}
+
 int fg_encoded_ltsv_stops(const fg_ctx* c, const int32_t** stop) {
     if (!c || !stop || c->enc_stop_n < 0) return FG_E_ARG;
     *stop = c->enc_stop.h;
@@ -1606,6 +1633,12 @@ int fg_split_decode_encode_capnp(fg_ctx* c, fg_format fmt, fg_framing framing, c
     return split_decode_encode(c, ENC_CAPNP, fmt, framing, stream, nbytes, out, line_offsets);
 }
 
+// framing + decode + PassthroughEncoder::encode on the device, as fg_split_decode_encode_gelf
+int fg_split_decode_encode_passthrough(fg_ctx* c, fg_format fmt, fg_framing framing, const uint8_t* stream, int64_t nbytes,
+                                       fg_encoded_out* out, const int32_t** line_offsets) {
+    return split_decode_encode(c, ENC_PASSTHROUGH, fmt, framing, stream, nbytes, out, line_offsets);
+}
+
 int fg_upload(fg_ctx* c, const uint8_t* bytes, const int32_t* offsets, int32_t n) {
     if (int rc = check_batch(c, bytes, offsets, n)) return rc;
     FG_CUDA(c, cudaSetDevice(c->device));
@@ -1686,6 +1719,7 @@ int fg_flush_l2(fg_ctx* c) {
 }
 
 const char* fg_error_string(fg_format, uint32_t status) {
+    if (status == FG_EP_NO_RAW) return "Cannot output empty raw message";  // encoder/passthrough_encoder.rs:44
     if (status == 0 || status >= FG_ST_COUNT) return nullptr;
     return kErrorStrings[status];
 }

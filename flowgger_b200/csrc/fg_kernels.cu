@@ -25,6 +25,8 @@ cudaError_t configure_kernels(int max_tile5424) {
     if (e != cudaSuccess) return e;
     e = configure_capnp_encode(max_tile5424);
     if (e != cudaSuccess) return e;
+    e = configure_passthrough_encode();
+    if (e != cudaSuccess) return e;
     e = configure_parse_ltsv(kLtsvMaxTile);
     if (e != cudaSuccess) return e;
     e = configure_parse_gelf(kGelfMaxTile);
@@ -59,7 +61,7 @@ cudaError_t launch_parse(int fmt, const ParseParams& p, cudaStream_t stream) {
 
 const char* kernel_build_info() {
     return "flowgger_b200 parse kernels: sm_90a, structural bitmaps + bit-walk over TMA-bulk-staged CTA tiles, "
-           "kernels=[parse5424_kernel, post5424_kernel, gelf_size_kernel, gelf_write_kernel, ltsv_size_kernel, ltsv_write_kernel, capnp_size_kernel, capnp_write_kernel, parse_ltsv_kernel, parse_gelf_kernel, post_gelf_kernel, parse3164_kernel]";
+           "kernels=[parse5424_kernel, post5424_kernel, gelf_size_kernel, gelf_write_kernel, ltsv_size_kernel, ltsv_write_kernel, capnp_size_kernel, capnp_write_kernel, passthrough_size_kernel, passthrough_write_kernel, parse_ltsv_kernel, parse_gelf_kernel, post_gelf_kernel, parse3164_kernel]";
 }
 
 }  // namespace fg

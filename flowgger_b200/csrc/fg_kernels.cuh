@@ -210,6 +210,11 @@ cudaError_t launch_ltsv_encode(int fmt, const GelfEncodeParams& p, void* d_scan_
 // and static_key_off [2 n_static + 1] their bounds (sorted by key on the host); long_json_span receives the refusals.
 cudaError_t configure_capnp_encode(int max_tile_bytes);
 cudaError_t launch_capnp_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
+// ---- fused passthrough encoder over the same four decoders' results (fg_passthrough_encode.cu) ----------------------
+// The same parameters, except that static_blob holds the header (output.syslog_prepend_timestamp, formatted by the caller)
+// and n_static its length; tile_bytes is not used (the kernels stage no tile) and long_json_span is not read.
+cudaError_t configure_passthrough_encode();
+cudaError_t launch_passthrough_encode(int fmt, const GelfEncodeParams& p, void* d_scan_temp, size_t scan_temp_bytes, cudaStream_t stream);
 
 // RFC5424 (short lines, staged tile): 64-line CTAs — tile waits and barriers half as wide as with 128 lines
 #ifndef FG_R5_LINES  // other shapes build with -DFG_R5_LINES / -DFG_R5_MINB for A/B runs

@@ -61,5 +61,8 @@ enum FgStatus : uint32_t {
     FG_E3_WITH_YEAR = 84,      // three date tokens that do not parse without a year
     FG_E3_DATE = 85,
     FG_E3_PANIC = 86,          // `_log_tokens[0]` on an empty Vec (:64): the reference thread panics
-    FG_ST_COUNT = 87
+    FG_ST_COUNT = 87,          // decoder and framing statuses are 1 .. FG_ST_COUNT - 1 (fg_error_count)
+    // Encoder statuses lie above every decoder status: an encoder's Err for a Record the decoder accepted.
+    // passthrough encoder (encoder/passthrough_encoder.rs:44): a Record without full_msg (only GELF input has one)
+    FG_EP_NO_RAW = 128
 };

@@ -242,6 +242,8 @@ const FusedCalls kFusedCalls[] = {
      fg_split_decode_encode_ltsv},
     {"fg_set_capnp_extra: ", fg_set_capnp_extra, "fg_decode_encode_capnp: ", fg_decode_encode_capnp, "fg_split_decode_encode_capnp: ",
      fg_split_decode_encode_capnp},
+    {"fg_set_passthrough_prefix: ", nullptr, "fg_decode_encode_passthrough: ", fg_decode_encode_passthrough,
+     "fg_split_decode_encode_passthrough: ", fg_split_decode_encode_passthrough},
 };
 const FusedCalls& fused_calls(const CudaFusedEncoder& enc) { return kFusedCalls[(int)enc.output()]; }
 }  // namespace
@@ -250,6 +252,13 @@ void CudaBatchDecoder::set_encoder(const CudaFusedEncoder& enc) {
     // set on every call: a host-side setting, and other callers of the same context may have changed it
     if (fg_set_output_framing(ctx_, enc.out_framing()) != FG_OK)
         throw std::runtime_error(std::string("fg_set_output_framing: ") + fg_last_error(ctx_));
+    const FusedCalls& f = fused_calls(enc);
+    if (enc.output() == CudaFusedEncoder::Output::Passthrough) {  // the header of this call, set on every call
+        const std::string h = enc.header() ? enc.header()() : std::string();
+        if (fg_set_passthrough_prefix(ctx_, (const uint8_t*)h.data(), (int64_t)h.size()) != FG_OK)
+            throw std::runtime_error(std::string(f.set_extra_name) + fg_last_error(ctx_));
+        return;
+    }
     const std::vector<std::pair<std::string, std::string>>& extra = enc.extra();
     const int o = (int)enc.output();
     if (extra_valid_[o] && extra == extra_set_[o]) return;
@@ -258,7 +267,6 @@ void CudaBatchDecoder::set_encoder(const CudaFusedEncoder& enc) {
         k.push_back(kv.first.c_str());
         v.push_back(kv.second.c_str());
     }
-    const FusedCalls& f = fused_calls(enc);
     if (f.set_extra(ctx_, (int32_t)extra.size(), k.data(), v.data()) != FG_OK)
         throw std::runtime_error(std::string(f.set_extra_name) + fg_last_error(ctx_));
     extra_set_[o] = extra;
@@ -1288,6 +1296,24 @@ int fgh_splitter_run_capnp_framed(void* d, const uint8_t* text, int64_t len, int
     std::string stream, err, out;
     auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
     const CudaCapnpEncoder enc(extra_of(n_extra, keys, vals), (fg_out_framing)out_framing);
+    if (run_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
+    give(stream, out_stream, out_stream_len);
+    give(err, out_stderr, out_stderr_len);
+    give(out, out_stdout, out_stdout_len);
+    return 0;
+}
+
+// fgh_splitter_run_gelf_framed with output.format = "passthrough" (CudaPassthroughEncoder): `header` [header_len] is
+// the header of every device call, none when NULL
+int fgh_splitter_run_passthrough_framed(void* d, const uint8_t* text, int64_t len, int32_t max_lines, int64_t max_bytes,
+                                        const uint8_t* header, int64_t header_len, int framing, int out_framing, uint8_t** out_stream,
+                                        int64_t* out_stream_len, uint8_t** out_stderr, int64_t* out_stderr_len, uint8_t** out_stdout,
+                                        int64_t* out_stdout_len) {
+    std::string stream, err, out;
+    auto tx = [&](std::vector<uint8_t>&& v) { stream.append(v.begin(), v.end()); };
+    std::function<std::string()> source;
+    if (header) source = [h = std::string((const char*)header, (size_t)header_len)] { return h; };
+    const CudaPassthroughEncoder enc(std::move(source), (fg_out_framing)out_framing);
     if (run_splitter(d, text, len, max_lines, max_bytes, framing, enc, tx, err, out)) return -1;
     give(stream, out_stream, out_stream_len);
     give(err, out_stderr, out_stderr_len);

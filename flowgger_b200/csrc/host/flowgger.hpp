@@ -200,7 +200,7 @@ class Encoder {
 // to run it on the device (CudaBatchDecoder::decode_encode / try_split_decode_encode).
 class CudaFusedEncoder : public Encoder {
    public:
-    enum class Output { Gelf, Ltsv, Capnp };
+    enum class Output { Gelf, Ltsv, Capnp, Passthrough };
     // the decoders whose device-resident results the fused encoders read
     static bool fuses_with(fg_format fmt) {
         return fmt == FG_FMT_RFC5424 || fmt == FG_FMT_RFC3164 || fmt == FG_FMT_LTSV || fmt == FG_FMT_GELF;
@@ -209,7 +209,8 @@ class CudaFusedEncoder : public Encoder {
     bool encode(Record&&, std::vector<uint8_t>&, const char** err) const override {
         static const char* const kWhat[] = {"GelfEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)",
                                             "LTSVEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)",
-                                            "CapnpEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)"};
+                                            "CapnpEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)",
+                                            "PassthroughEncoder runs fused with the decoder on the GPU (use BatchingLineSplitter)"};
         if (err) *err = kWhat[(int)output_];
         return false;
     }
@@ -217,15 +218,19 @@ class CudaFusedEncoder : public Encoder {
     // output.gelf_extra, output.ltsv_extra or output.capnp_extra
     const std::vector<std::pair<std::string, std::string>>& extra() const { return extra_; }
     fg_out_framing out_framing() const { return out_framing_; }
+    // Output::Passthrough: the header of the records of one device call, asked once per call (none: no header)
+    const std::function<std::string()>& header() const { return header_; }
 
    protected:
-    CudaFusedEncoder(Output output, std::vector<std::pair<std::string, std::string>> extra, fg_out_framing out_framing)
-        : output_(output), extra_(std::move(extra)), out_framing_(out_framing) {}
+    CudaFusedEncoder(Output output, std::vector<std::pair<std::string, std::string>> extra, fg_out_framing out_framing,
+                     std::function<std::string()> header = {})
+        : output_(output), extra_(std::move(extra)), out_framing_(out_framing), header_(std::move(header)) {}
 
    private:
     Output output_;
     std::vector<std::pair<std::string, std::string>> extra_;
     fg_out_framing out_framing_;
+    std::function<std::string()> header_;
 };
 
 class CudaGelfEncoder : public CudaFusedEncoder {
@@ -250,6 +255,18 @@ class CudaCapnpEncoder : public CudaFusedEncoder {
    public:
     explicit CudaCapnpEncoder(std::vector<std::pair<std::string, std::string>> extra = {}, fg_out_framing out_framing = FG_OUT_NONE)
         : CudaFusedEncoder(Output::Capnp, std::move(extra), out_framing) {}
+};
+
+// encoder/passthrough_encoder.rs:10-46: output.format = "passthrough", fused with the decoder on the GPU as
+// CudaGelfEncoder is (fg_decode_encode_passthrough): each record is the header + Record.full_msg.  `header` =
+// output.syslog_prepend_timestamp formatted for the current time, called once per device call before it runs (none: no
+// header); `out_framing` = output.framing, resolved by the caller (the reference's default: "noop", FG_OUT_NONE, and
+// "line" for output.type = "debug", mod.rs:444-451).  A GELF record without full_message gets the encoder's error
+// (FG_EP_NO_RAW) on stderr, as a decoder error.
+class CudaPassthroughEncoder : public CudaFusedEncoder {
+   public:
+    explicit CudaPassthroughEncoder(std::function<std::string()> header = {}, fg_out_framing out_framing = FG_OUT_NONE)
+        : CudaFusedEncoder(Output::Passthrough, {}, out_framing, std::move(header)) {}
 };
 
 // What RecordBatcher and the batching splitters do with each record of a batch decoded on the device, one record at a

@@ -113,6 +113,9 @@ def load_cuda() -> C.CDLL:
         L.fg_set_capnp_extra.argtypes = L.fg_set_ltsv_extra.argtypes
         L.fg_decode_encode_capnp.argtypes = L.fg_decode_encode_gelf.argtypes
         L.fg_split_decode_encode_capnp.argtypes = L.fg_split_decode_encode_gelf.argtypes
+        L.fg_set_passthrough_prefix.argtypes = [C.c_void_p, C.c_char_p, C.c_int64]
+        L.fg_decode_encode_passthrough.argtypes = L.fg_decode_encode_gelf.argtypes
+        L.fg_split_decode_encode_passthrough.argtypes = L.fg_split_decode_encode_gelf.argtypes
         L.fg_encoded_ltsv_stops.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int32))]
         L.fg_encoded_gelf_now.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
         L.fg_set_output_framing.argtypes = [C.c_void_p, C.c_int]
@@ -156,6 +159,8 @@ def load_host() -> C.CDLL:
                                                    C.POINTER(C.c_char_p), C.c_int, C.c_int] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         L.fgh_splitter_run_ltsv_framed.argtypes = L.fgh_splitter_run_gelf_framed.argtypes
         L.fgh_splitter_run_capnp_framed.argtypes = L.fgh_splitter_run_gelf_framed.argtypes
+        L.fgh_splitter_run_passthrough_framed.argtypes = [C.c_void_p, C.c_char_p, C.c_int64, C.c_int32, C.c_int64, C.c_char_p, C.c_int64,
+                                                          C.c_int, C.c_int] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         L.fgh_splitter_run.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int64, C.c_int32, C.c_int64] + [C.POINTER(C.c_void_p), C.POINTER(C.c_int64)] * 3
         _host = L
     return _host
@@ -456,6 +461,22 @@ class BatchDecoder:
         """split_decode_encode_gelf with the Cap'n Proto encoder (fg_split_decode_encode_capnp)."""
         return self._split_decode_encode("fg_split_decode_encode_capnp", stream, framing, copy)
 
+    def set_passthrough_prefix(self, header: bytes) -> None:
+        """The header of the following passthrough calls (output.syslog_prepend_timestamp, formatted by the caller), written
+        as given; b"" clears it."""
+        self._check(self.L.fg_set_passthrough_prefix(self.ctx, header, len(header)), "fg_set_passthrough_prefix")
+
+    def decode_encode_passthrough(self, data: np.ndarray, offsets: np.ndarray, copy: bool = True):
+        """decode + PassthroughEncoder::encode fused on the device (fg_decode_encode_passthrough), for the same four
+        decoders as decode_encode_gelf and with the same results: (records, int64 offsets[n+1], status uint8[n], kernel ms).
+        Record i is the header + Record.full_msg; a GELF object without full_message has status FG_EP_NO_RAW and no
+        record.  The default output.framing of passthrough is none ("noop"), "line" for output.type = "debug"."""
+        return self._decode_encode("fg_decode_encode_passthrough", data, offsets, copy)
+
+    def split_decode_encode_passthrough(self, stream: np.ndarray, framing: int = 0, copy: bool = True):
+        """split_decode_encode_gelf with the passthrough encoder (fg_split_decode_encode_passthrough)."""
+        return self._split_decode_encode("fg_split_decode_encode_passthrough", stream, framing, copy)
+
     def _decode_encode(self, fn: str, data: np.ndarray, offsets: np.ndarray, copy: bool):
         assert data.dtype == np.uint8 and offsets.dtype == np.int32
         out = FgEncodedOut()
@@ -681,6 +702,16 @@ def splitter_run_capnp_framed(dec: "BatchDecoder", text: bytes, out_framing: int
     n_extra, keys, vals = _extra_arrays(extra)
     return _run_splitter(lambda o: H.fgh_splitter_run_capnp_framed(dec._h, text, len(text), max_lines, max_bytes, n_extra, keys,
                                                                    vals, framing, out_framing, *o))
+
+
+def splitter_run_passthrough_framed(dec: "BatchDecoder", text: bytes, out_framing: int = 0, header: bytes | None = None,
+                                    max_lines: int = 1 << 16, max_bytes: int = 16 << 20, framing: int = 0) -> tuple[bytes, bytes, bytes]:
+    """splitter_run_gelf_framed with output.format = "passthrough" (CudaPassthroughEncoder, whose header source gives
+    `header` for every device call, none when None; output.framing defaults to none, the reference's "noop"): returns (the
+    output stream exactly as the splitter sent it, stderr text, stdout text)."""
+    H = load_host()
+    return _run_splitter(lambda o: H.fgh_splitter_run_passthrough_framed(dec._h, text, len(text), max_lines, max_bytes, header,
+                                                                         len(header or b""), framing, out_framing, *o))
 
 
 def splitter_run(dec: "BatchDecoder", text: bytes, max_lines: int = 1 << 16, max_bytes: int = 16 << 20,

@@ -351,6 +351,28 @@ int fg_decode_encode_capnp(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT
                            const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
 int fg_split_decode_encode_capnp(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */, fg_framing framing,
                                  const uint8_t* stream, int64_t nbytes, fg_encoded_out* out, const int32_t** line_offsets);
+/* output.format = "passthrough" (encoder/passthrough_encoder.rs:10-46), the same four input formats:
+ *     PassthroughEncoder::new(&Config)  passthrough_encoder.rs:11-14  -> fg_set_passthrough_prefix (the header)
+ *     Encoder::encode(Record)           passthrough_encoder.rs:22-46  -> fg_decode_encode_passthrough /
+ *                                                                         fg_split_decode_encode_passthrough
+ * Record i is the header followed by Record.full_msg, byte for byte: for RFC5424 input the line after its BOM with
+ * trailing Unicode White_Space removed, for RFC3164 the whole line (<PRI> included) trimmed the same way, for LTSV the
+ * line as given, for GELF the unescaped full_message string ("" gives an accepted, empty record).  A GELF object without
+ * full_message is the encoder's error: status FG_EP_NO_RAW = 128 (fg_error_string: "Cannot output empty raw message"), an
+ * empty record and no frame, as a decoder error.  Everything else — fg_encoded_out, statuses, empty rejected records,
+ * output.framing (the caller resolves the reference's default: "noop", FG_OUT_NONE, except "line" for output.type =
+ * "debug"), fg_encoded_ltsv_stops, fg_encoded_gelf_now, FG_E_CAPACITY, the input format rule — is exactly as for the
+ * GELF twins above.
+ * fg_set_passthrough_prefix: the header of the following passthrough calls, written as given (any bytes, NUL and '\n'
+ * included).  The reference formats output.syslog_prepend_timestamp per record (encoder/mod.rs:58-94); here the caller
+ * formats it once per call (see fg_encoded_gelf_now for the same trade).  n = 0 clears it; NULL bytes with n > 0, or
+ * n >= 2^31 -> FG_E_ARG with the header unchanged. */
+int fg_set_passthrough_prefix(fg_ctx* ctx, const uint8_t* bytes, int64_t n);
+int fg_decode_encode_passthrough(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */,
+                                 const uint8_t* bytes, const int32_t* offsets, int32_t n, fg_encoded_out* out);
+int fg_split_decode_encode_passthrough(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | FG_FMT_RFC3164 | FG_FMT_LTSV | FG_FMT_GELF */,
+                                       fg_framing framing, const uint8_t* stream, int64_t nbytes, fg_encoded_out* out,
+                                       const int32_t** line_offsets);
 /* The one side effect of LTSVDecoder::decode, println!("Missing value for name '{}'") for every tab-separated part
  * without ':' that the decode loop reached (ltsv_decoder.rs:99), for the records of the last fused call on an LTSV
  * context.  *stop ([out->n], valid until the next call on the context): -1 when record i printed nothing; else the offset,
@@ -361,10 +383,16 @@ int fg_split_decode_encode_capnp(fg_ctx* ctx, fg_format fmt /* FG_FMT_RFC5424 | 
 int fg_encoded_ltsv_stops(const fg_ctx* ctx, const int32_t** stop);
 /* Record.ts of every record without "timestamp" in the last fused call on GELF input: CLOCK_REALTIME at the start of
  * that call, as secs + nanos / 1e9 (utils/mod.rs:16-21).  Returns FG_E_ARG when the last fused call was not on GELF
- * input or failed. */
+ * input or failed.
+ * The passthrough header (fg_set_passthrough_prefix) makes the same trade: the reference formats
+ * output.syslog_prepend_timestamp from OffsetDateTime::now_utc() per record, the device writes one header per call.  The
+ * two differ only for the records the reference would have encoded after the clock crossed a tick of the format's
+ * finest field (a second, a minute, ...) during the call. */
 int fg_encoded_gelf_now(const fg_ctx* ctx, double* now);
 
-/* the reference's Err(&'static str) for a row status (0 -> NULL) */
+/* the reference's Err(&'static str) for a row status (0 -> NULL).  fg_error_count: one past the largest status a decoder
+ * or the framing gives; an encoder's status lies above every one of them (FG_EP_NO_RAW = 128, the passthrough encoder's
+ * "Cannot output empty raw message"). */
 const char* fg_error_string(fg_format fmt, uint32_t status);
 uint32_t fg_error_count(void);
 

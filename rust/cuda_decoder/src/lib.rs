@@ -13,7 +13,7 @@
 
 use flowgger::flowgger::config::Config;
 use flowgger::flowgger::decoder::Decoder;
-use flowgger::flowgger::encoder::Encoder;
+use flowgger::flowgger::encoder::{build_prepend_ts, config_get_prepend_ts, Encoder};
 use flowgger::flowgger::record::{Record, SDValue, StructuredData};
 use flowgger::flowgger::splitter::Splitter;
 use std::ffi::{CStr, CString};
@@ -224,19 +224,23 @@ impl CudaDecoder {
     /// call, the bytes one Output writes for them.  false (nothing decoded) when the stream does not fit the context.
     pub fn split_decode_encode_gelf<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String]), G: FnOnce(&[u8])>(
         &self, stream: &[u8], extra: &[(String, String)], out_framing: fg_out_framing, f: F, all: G) -> bool {
-        self.split_decode_encode(FusedOutput::Gelf, stream, extra, out_framing, f, all)
+        self.split_decode_encode(FusedOutput::Gelf, stream, extra, &[], out_framing, f, all)
     }
 
     /// `split_decode_encode_gelf` for any fused encoder: `output` = output.format, `extra` = its extras
     /// (output.gelf_extra, output.ltsv_extra or output.capnp_extra); with `FusedOutput::Ltsv` the records are
     /// `LTSVEncoder::encode`'s text (`fg_split_decode_encode_ltsv`), with `FusedOutput::Capnp` `CapnpEncoder::encode`'s
-    /// messages (`fg_split_decode_encode_capnp`).
+    /// messages (`fg_split_decode_encode_capnp`), with `FusedOutput::Passthrough` `prefix` + Record.full_msg
+    /// (`fg_split_decode_encode_passthrough`; `prefix` is the header of this call, `extra` is not used).
     pub fn split_decode_encode<F: FnMut(&[u8], Result<&[u8], &'static str>, &[String]), G: FnOnce(&[u8])>(
-        &self, output: FusedOutput, stream: &[u8], extra: &[(String, String)], out_framing: fg_out_framing, mut f: F, all: G) -> bool {
+        &self, output: FusedOutput, stream: &[u8], extra: &[(String, String)], prefix: &[u8], out_framing: fg_out_framing, mut f: F,
+        all: G) -> bool {
         let mut ctx = self.ctx.lock().unwrap();
         assert_eq!(unsafe { fg_set_output_framing(ctx.raw, out_framing) }, 0);
         let o = output as usize;
-        if ctx.extra[o].as_deref() != Some(extra) {
+        if output == FusedOutput::Passthrough {  // set on every call: the header carries the time of the call
+            assert_eq!(unsafe { fg_set_passthrough_prefix(ctx.raw, prefix.as_ptr(), prefix.len() as i64) }, 0);
+        } else if ctx.extra[o].as_deref() != Some(extra) {
             let keys: Vec<CString> = extra.iter().map(|(k, _)| CString::new(k.as_str()).unwrap()).collect();
             let vals: Vec<CString> = extra.iter().map(|(_, v)| CString::new(v.as_str()).unwrap()).collect();
             let kp: Vec<*const c_char> = keys.iter().map(|s| s.as_ptr()).collect();
@@ -245,6 +249,7 @@ impl CudaDecoder {
                 FusedOutput::Gelf => fg_set_gelf_extra,
                 FusedOutput::Ltsv => fg_set_ltsv_extra,
                 FusedOutput::Capnp => fg_set_capnp_extra,
+                FusedOutput::Passthrough => unreachable!(),
             };
             assert_eq!(unsafe { set(ctx.raw, kp.len() as i32, kp.as_ptr(), vp.as_ptr()) }, 0);
             ctx.extra[o] = Some(extra.to_vec());
@@ -255,6 +260,7 @@ impl CudaDecoder {
             FusedOutput::Gelf => fg_split_decode_encode_gelf,
             FusedOutput::Ltsv => fg_split_decode_encode_ltsv,
             FusedOutput::Capnp => fg_split_decode_encode_capnp,
+            FusedOutput::Passthrough => fg_split_decode_encode_passthrough,
         };
         let rc = unsafe { call(ctx.raw, ctx.fmt, fg_framing_FG_FRAME_LINE, stream.as_ptr(), stream.len() as i64, &mut out, &mut lines) };
         if rc == FG_E_CAPACITY {
@@ -619,12 +625,20 @@ pub fn fuses_with_capnp(input_format: &str) -> bool {
     fuses_with_gelf(input_format)
 }
 
-/// The output format of a fused encoder (output.format = "gelf", "ltsv" or "capnp")
+/// The `input.format` values whose decoder runs fused with the passthrough encoder on the device
+/// (`fg_decode_encode_passthrough`, `fg_split_decode_encode_passthrough`): the same four;
+/// `FusedPassthroughLineSplitter` takes a `CudaDecoder` of one of them.
+pub fn fuses_with_passthrough(input_format: &str) -> bool {
+    fuses_with_gelf(input_format)
+}
+
+/// The output format of a fused encoder (output.format = "gelf", "ltsv", "capnp" or "passthrough")
 #[derive(Clone, Copy, PartialEq, Eq, Debug)]
 pub enum FusedOutput {
     Gelf = 0,
     Ltsv = 1,
     Capnp = 2,
+    Passthrough = 3,
 }
 
 /// The device framing of an `output.framing` value, as `mod.rs:453-460` picks the merger (panics on an unknown one, as
@@ -657,7 +671,7 @@ pub struct FusedGelfLineSplitter {
 
 impl<T: Read> Splitter<T> for FusedGelfLineSplitter {
     fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
-        run_fused(&self.gpu, FusedOutput::Gelf, &self.extra, self.out_framing, self.max_bytes, buf_reader, tx)
+        run_fused(&self.gpu, FusedOutput::Gelf, &self.extra, None, self.out_framing, self.max_bytes, buf_reader, tx)
     }
 }
 
@@ -673,7 +687,7 @@ pub struct FusedLtsvLineSplitter {
 
 impl<T: Read> Splitter<T> for FusedLtsvLineSplitter {
     fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
-        run_fused(&self.gpu, FusedOutput::Ltsv, &self.extra, self.out_framing, self.max_bytes, buf_reader, tx)
+        run_fused(&self.gpu, FusedOutput::Ltsv, &self.extra, None, self.out_framing, self.max_bytes, buf_reader, tx)
     }
 }
 
@@ -689,17 +703,53 @@ pub struct FusedCapnpLineSplitter {
 
 impl<T: Read> Splitter<T> for FusedCapnpLineSplitter {
     fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
-        run_fused(&self.gpu, FusedOutput::Capnp, &self.extra, self.out_framing, self.max_bytes, buf_reader, tx)
+        run_fused(&self.gpu, FusedOutput::Capnp, &self.extra, None, self.out_framing, self.max_bytes, buf_reader, tx)
     }
 }
 
-fn run_fused<T: Read>(gpu: &CudaDecoder, output: FusedOutput, extra: &[(String, String)], out_framing: fg_out_framing, max_bytes: usize,
-                      buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>) {
+/// `output.format = "passthrough"` with `input.format` one of `fuses_with_passthrough`: `FusedGelfLineSplitter` with the
+/// passthrough encoder (`fg_split_decode_encode_passthrough`, replaces Decoder::decode + PassthroughEncoder::encode,
+/// passthrough_encoder.rs:22-46): each record is the header + Record.full_msg, and a GELF record without full_message
+/// prints "Cannot output empty raw message: [line]" on stderr.  The header (output.syslog_prepend_timestamp) is
+/// formatted once per device call, as build_prepend_ts does per record (encoder/mod.rs:82-94), so it can differ from
+/// the reference's for the records encoded after the clock crossed a tick of the format's finest field during the call.
+/// The caller resolves output.framing's default (mod.rs:444-451): "noop", `FG_OUT_NONE`, or "line" for output.type =
+/// "debug".
+pub struct FusedPassthroughLineSplitter {
+    pub gpu: CudaDecoder,
+    pub header_format: Option<String>,  // config_get_prepend_ts (encoder/mod.rs:58-80): validated, None without a header
+    pub out_framing: fg_out_framing,    // output.framing (mod.rs:444-451), resolved by the caller
+    pub max_bytes: usize,
+}
+
+impl FusedPassthroughLineSplitter {
+    /// None when output.syslog_prepend_timestamp is not a format description build_prepend_ts can use: the reference
+    /// then fails every record that has a full_msg ("Failed to format date when building prepend timestamp for header
+    /// while encoding Passthrough"), which the caller keeps by running LineSplitter with PassthroughEncoder instead.
+    pub fn new(gpu: CudaDecoder, config: &Config, out_framing: fg_out_framing, max_bytes: usize) -> Option<FusedPassthroughLineSplitter> {
+        let header_format = config_get_prepend_ts(config);
+        if let Some(f) = &header_format {
+            build_prepend_ts(f).ok()?;
+        }
+        Some(FusedPassthroughLineSplitter { gpu, header_format, out_framing, max_bytes })
+    }
+}
+
+impl<T: Read> Splitter<T> for FusedPassthroughLineSplitter {
+    fn run(&self, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>, _decoder: Box<dyn Decoder>, _encoder: Box<dyn Encoder>) {
+        run_fused(&self.gpu, FusedOutput::Passthrough, &[], self.header_format.as_deref(), self.out_framing, self.max_bytes, buf_reader, tx)
+    }
+}
+
+fn run_fused<T: Read>(gpu: &CudaDecoder, output: FusedOutput, extra: &[(String, String)], header_format: Option<&str>,
+                      out_framing: fg_out_framing, max_bytes: usize, buf_reader: BufReader<T>, tx: SyncSender<Vec<u8>>) {
     let max_bytes = max_bytes.min(gpu.capacity_bytes());
     let framed = out_framing != fg_out_framing_FG_OUT_NONE;
     run_blocks(buf_reader, max_bytes, |block| {
         decode_fitting(gpu, block, &mut |gpu: &CudaDecoder, part: &[u8]| {
-            gpu.split_decode_encode(output, part, extra, out_framing, |line, r, side| {
+            // the passthrough header of this device call (FusedPassthroughLineSplitter::new checked that it formats)
+            let prefix = header_format.map_or(String::new(), |f| build_prepend_ts(f).expect("syslog_prepend_timestamp"));
+            gpu.split_decode_encode(output, part, extra, prefix.as_bytes(), out_framing, |line, r, side| {
                 for s in side { println!("{}", s); }  // ltsv_decoder.rs:99
                 match r {
                     Ok(rec) => if !framed { tx.send(rec.to_vec()).unwrap() },

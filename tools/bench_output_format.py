@@ -1,6 +1,7 @@
-"""GELF, LTSV and Cap'n Proto output side by side on the device, per input format: output.format = "gelf"
-(fg_decode_encode_gelf), "ltsv" (fg_decode_encode_ltsv) and "capnp" (fg_decode_encode_capnp) over the same pre-framed
-lines in pinned memory, timed alternately in one process.
+"""GELF, LTSV, Cap'n Proto and passthrough output side by side on the device, per input format: output.format = "gelf"
+(fg_decode_encode_gelf), "ltsv" (fg_decode_encode_ltsv), "capnp" (fg_decode_encode_capnp) and "passthrough"
+(fg_decode_encode_passthrough, no header) over the same pre-framed lines in pinned memory, timed alternately in one
+process.
 
     python tools/bench_output_format.py [--lines 4000000] [--steps 10] [--warmup 2] [--formats rfc5424,rfc3164,ltsv,gelf]
 
@@ -41,7 +42,8 @@ def main() -> None:
         data[:] = lines
         offs = dec.host_alloc(4 * len(loffs), np.int32)
         offs[:] = loffs
-        calls = {"gelf": dec.decode_encode_gelf, "ltsv": dec.decode_encode_ltsv, "capnp": dec.decode_encode_capnp}
+        calls = {"gelf": dec.decode_encode_gelf, "ltsv": dec.decode_encode_ltsv, "capnp": dec.decode_encode_capnp,
+                 "passthrough": dec.decode_encode_passthrough}
         km = {k: [] for k in calls}
         wall = {k: [] for k in calls}
         nbytes = {}
