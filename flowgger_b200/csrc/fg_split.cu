@@ -79,14 +79,16 @@ __global__ void __launch_bounds__(1024) scan_segments_kernel(uint32_t* __restric
     if (t == 1023) {
         const unsigned long long newlines = (unsigned long long)before + part[1023];
         *run = (uint32_t)newlines;
-        const bool over = newlines + 1ull > (unsigned long long)max_lines;
+        // records so far: bytes follow a chunk that is not the last, so one more record is open after it; after the last
+        // chunk only an unterminated last record counts (BufRead::lines / split yield it), a terminated one has no successor
+        const bool tail = is_last && nbytes > 0 && bytes[nbytes - 1] != delim;
+        const unsigned long long n = newlines + (is_last ? (tail ? 1ull : 0ull) : 1ull);
+        const bool over = n > (unsigned long long)max_lines;
         *cum_out = over ? -1 : (int32_t)newlines;
         if (seg0 == 0) offsets[0] = 0;
         if (is_last) {
-            const bool tail = nbytes > 0 && bytes[nbytes - 1] != delim;  // BufRead::lines / split yield an unterminated last record
-            const long long n = (long long)newlines + (tail ? 1 : 0);
-            *n_lines = (over || n > max_lines) ? -1 : (int32_t)n;
-            if (!over && n <= max_lines && tail) offsets[n] = (int32_t)nbytes;
+            *n_lines = over ? -1 : (int32_t)n;
+            if (!over && tail) offsets[n] = (int32_t)nbytes;
         }
     }
 }

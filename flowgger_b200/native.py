@@ -93,6 +93,7 @@ def load_cuda() -> C.CDLL:
         L.fg_host_alloc.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p)]
         L.fg_host_free.argtypes = [C.c_void_p, C.c_void_p]
         L.fg_split_decode.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.POINTER(FgBatchOut)]
+        L.fg_split_decode_framed.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.POINTER(FgBatchOut)]
         L.fg_last_split_ms.restype = C.c_float
         L.fg_last_split_ms.argtypes = [C.c_void_p]
         L.fg_error_count.restype = C.c_uint32
@@ -527,12 +528,18 @@ class BatchDecoder:
         self._check(self.L.fg_encoded_gelf_now(self.ctx, C.byref(v)), "fg_encoded_gelf_now")
         return v.value
 
-    def split_decode(self, stream: np.ndarray) -> BatchResult:
-        """Framing + UTF-8 validation + decode of a raw newline-terminated byte stream, all on the device."""
+    def split_decode(self, stream: np.ndarray, framing: int | None = None) -> BatchResult:
+        """Framing + UTF-8 validation + decode of a raw byte stream, all on the device: fg_split_decode (newline
+        framing), or fg_split_decode_framed with `framing` 0 = "line", 1 = "nul".  The record starts, n + 1 int32, are at
+        BatchResult.raw.line_offsets."""
         assert stream.dtype == np.uint8
         out = FgBatchOut()
         self._keep = (stream,)
-        self._check(self.L.fg_split_decode(self.ctx, self.fmt, _ptr(stream), len(stream), C.byref(out)), "fg_split_decode")
+        if framing is None:
+            self._check(self.L.fg_split_decode(self.ctx, self.fmt, _ptr(stream), len(stream), C.byref(out)), "fg_split_decode")
+        else:
+            self._check(self.L.fg_split_decode_framed(self.ctx, self.fmt, framing, _ptr(stream), len(stream), C.byref(out)),
+                        "fg_split_decode_framed")
         return BatchResult(out, self.fmt)
 
     def last_split_ms(self) -> float:
